@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of sourmash_b200 (contract: see the task statement / DESIGN.md §Measurement).
+"""bench.py -- headline benchmark of sourmash_b200 on one H100 (see DESIGN.md §Measurement).
 
 Primary workload (BASELINE.json configs[2]): `compare` of 10 000 synthetic FracMinHash sketches
 (k=31, scaled=1000, ~5000 hashes each, 100 families) -> all-vs-all Jaccard matrix; metric
@@ -11,6 +11,8 @@ k=21,31,51 scaled=1000 over 100 synthetic 5 Mbp genomes; metric k-mers hashed/s.
     python bench.py --impl reference ...                           # CPU restatement on host cores
 
 One JSON line on stdout (rank 0).  Only the cpu_baseline / --impl reference legs touch oracle/.
+--dump-outputs DIR writes what the last timed step computed as DIR/<name>.npy (float64, <= 64 MB in all), so that
+two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -32,13 +34,36 @@ COMPARE_WORKLOAD = ("configs[2]: compare 10000 synthetic sketches (k=31, scaled=
                     "100 families) all-vs-all jaccard float64 matrix")
 SKETCH_WORKLOAD = "configs[1]: sketch dna k=21,31,51 scaled=1000 on 100 synthetic 5 Mbp genomes"
 N_DB_SEARCH, N_DB_GATHER, N_QUERY_SEARCH = 300_000, 50_000, 10_000_000   # configs[3] / configs[4] shapes
-SM_COUNT = 148                                        # B200
+SM_COUNT = 132                                        # H100 SXM
 GENOME_LEN = 5_000_000
 SCALED = 1000
 
 
 def log(*a):
     print(*a, file=sys.stderr, flush=True)
+
+
+# --dump-outputs: arrays of the last timed step, by file name; a fixed, seeded sample where the whole output is larger
+DUMP = {}
+DUMP_LIMIT_BYTES = 64 << 20
+DUMP_COMPARE_ROWS = 256                               # of the 10 000 rows of the compare matrix: 20 MB of float64
+
+
+def dump_u64(name, a):
+    "u64 hashes exceed float64's 53-bit mantissa: stored exactly as their high and low 32-bit halves"
+    a = np.asarray(a, dtype=np.uint64)
+    DUMP[name + "_hi32"] = (a >> np.uint64(32)).astype(np.float64)
+    DUMP[name + "_lo32"] = (a & np.uint64(0xffffffff)).astype(np.float64)
+
+
+def write_dump(dirname):
+    total = sum(a.nbytes for a in DUMP.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_LIMIT_BYTES))
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in sorted(DUMP.items()):
+        np.save(os.path.join(dirname, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+    log(f"[bench] wrote {len(DUMP)} arrays ({total} bytes) to {dirname}")
 
 
 # stdout carries exactly one JSON line: keep a private handle to the real stdout and point fd 1
@@ -172,7 +197,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def git_blob_hash(path):
@@ -309,7 +334,7 @@ def bind_to_gpu_cpus(torch, local_rank):
         return "cpu affinity unchanged (%s)" % type(exc).__name__
 
 
-# ----------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------- GPU arm
 def run_b200(args):
     import torch
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -410,6 +435,10 @@ def bench_compare(args, torch, dist, B, rank, world, timed, hbm_peak, peak_src):
 
         ms, launches, clocks, _ = timed(step_prof, args.steps, args.warmup)
         kernel_ms = kernel_ms[-args.steps:]
+        if args.dump_outputs:
+            pick = np.sort(np.random.Generator(np.random.PCG64(0)).choice(n, size=min(n, DUMP_COMPARE_ROWS), replace=False))
+            DUMP["compare_row_ids"] = pick.astype(np.float64)
+            DUMP["compare_jaccard_rows"] = d_out[torch.from_numpy(pick).to(dev)].cpu().numpy()
         # end to end: host CSR (pinned) -> H2D -> kernels -> D2H of the float64 matrix (pinned)
         ph, po = B.pinned_empty(len(h), np.uint64), B.pinned_empty(len(off), np.uint64)
         ph.array[:] = h
@@ -471,7 +500,7 @@ def bench_compare(args, torch, dist, B, rank, world, timed, hbm_peak, peak_src):
         "scaling": "strong", "vs_baseline": None, "dtype": "u64", "data": "synthetic",
         "config": {"workload": COMPARE_WORKLOAD,
                    "n_sketches": n, "pairs_per_step": n_pairs, "parallelism": parallelism,
-                   "l2_policy": "inputs 400 MB + 800 MB output per step exceed the 126 MB L2; no flush"},
+                   "l2_policy": "inputs 400 MB + 800 MB output per step exceed the 50 MB L2; no flush"},
         "e2e": {"value": n_pairs / (ms_e2e / 1e3), "unit": "pairs/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": launches,
@@ -539,6 +568,10 @@ def bench_sketch(args, torch, dist, B, rank, world, timed, hbm_peak, peak_src):
 
     ms, launches, clocks, _ = timed(step, args.steps, args.warmup)
     kernel_ms = kernel_ms[-args.steps:]
+    if args.dump_outputs:                                 # rows: genome-major, k = 21, 31, 51 within a genome
+        hh, oo = last["sset"].to_host()
+        dump_u64("sketch_hashes", hh)
+        DUMP["sketch_row_offsets"] = oo.astype(np.float64)
     pin = B.pinned_empty(len(my_seqs), np.uint8)
     pin.array[:] = my_seqs
 
@@ -559,7 +592,7 @@ def bench_sketch(args, torch, dist, B, rank, world, timed, hbm_peak, peak_src):
         "config": {"workload": SKETCH_WORKLOAD,
                    "kmers_per_step": total_kmers,
                    "parallelism": "1 gpu" if world == 1 else f"{world} gpus: genomes round-robin, sketches all-gathered",
-                   "l2_policy": "500 MB of bases per pass exceed the 126 MB L2; no flush"},
+                   "l2_policy": "500 MB of bases per pass exceed the 50 MB L2; no flush"},
         "e2e": {"value": total_kmers / (ms_e2e / 1e3), "unit": "k-mers/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": int(len(my_seqs)), "d2h_bytes_per_step": int(ex[-1]) * 8},
         "gpu_launches": launches, "clocks": clocks,
@@ -578,7 +611,7 @@ def bench_sketch(args, torch, dist, B, rank, world, timed, hbm_peak, peak_src):
     if wipk:
         # the bound that applies: warp instructions issued (ncu count of the same three launches, per k-mer)
         # against 4 issue slots per SM per clock at the SM clock sampled during the timed region
-        clk = float((clocks or {}).get("sm_mhz") or 1965.0) * 1e6
+        clk = float((clocks or {}).get("sm_mhz") or 1980.0) * 1e6
         issued = wipk * my_kmers / (kms / 1e3)
         res["roofline"]["issue"] = {"warp_instructions_per_kmer": wipk, "achieved": issued / 1e9,
                                     "peak": SM_COUNT * 4 * clk / 1e9, "unit": "G warp-instr/s",
@@ -748,13 +781,15 @@ def _bench_search(args, torch, dist, B, rank, world, timed, query, db, d_h, h_of
         def step_e2e():
             return int(sdb.search_counts(pq.array).sum())
     ms, launches, clocks, _ = timed(step, args.steps, args.warmup)
+    if args.dump_outputs:
+        DUMP["search_counts"] = d_counts[: hi - lo].cpu().numpy().astype(np.float64)
     ms_e2e, _, _, ex = timed(step_e2e, max(2, args.steps // 2), 1)
     alg = 8.0 * (n_hashes_total + nq * world)                    # every database hash once; the query once per rank
     achieved = alg / (ms / 1e3) / 1e9
     res = {"metric": "subjects searched/sec (search: 1e7-hash query vs 300000-sketch database)", "value": n_db / (ms / 1e3),
            "unit": "subjects/s", "ms_per_step": ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
            "config": {"workload": SEARCH_WORKLOAD, "db_hashes": n_hashes_total, "query_hashes": nq, "parallelism": parallelism,
-                      "l2_policy": "12 GB streamed per pass: far beyond the 126 MB L2; no flush"},
+                      "l2_policy": "12 GB streamed per pass: far beyond the 50 MB L2; no flush"},
            "e2e": {"value": n_db / (ms_e2e / 1e3), "unit": "subjects/s", "ms_per_step": ms_e2e,
                    "h2d_bytes_per_step": int(query.nbytes), "d2h_bytes_per_step": int(4 * n_db)},
            "gpu_launches": launches, "clocks": clocks,
@@ -830,6 +865,9 @@ def _bench_gather(args, torch, dist, B, rank, world, timed, query, db, d_h, h_of
             return len(ids)
     ms, launches, clocks, ex = timed(step, args.steps, args.warmup)
     ids, isizes = res["picks"]
+    if args.dump_outputs:
+        DUMP["gather_rows"] = np.asarray(ids, dtype=np.float64)
+        DUMP["gather_intersections"] = np.asarray(isizes, dtype=np.float64)
     out = {"metric": "gather wall time (configs[4])", "value": ms, "unit": "ms", "higher_is_better": False, "ms_per_step": ms,
            "scaling": "strong", "vs_baseline": None,
            "config": {"workload": GATHER_WORKLOAD, "query_hashes": int(len(query)), "db_rows": n_db, "parallelism": parallelism},
@@ -864,7 +902,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--index", action="store_true",
                     help="search / gather workloads: query through the inverted index of the resident database")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "b200" or args.gpus != 1):
+        ap.error("--dump-outputs needs --impl b200 --gpus 1")
     if args.workload is None:
         args.workload = "compare" if args.impl == "reference" else "both"
     if args.warmup < 3 and args.impl == "b200":
@@ -874,6 +918,8 @@ def main():
         run_reference(args)
     else:
         run_b200(args)
+    if args.dump_outputs:
+        write_dump(args.dump_outputs)
 
 
 if __name__ == "__main__":

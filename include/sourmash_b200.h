@@ -1,9 +1,9 @@
 /*
- * sourmash_b200.h -- C ABI of libsourmash_b200.so, the B200 (sm_100a) implementation of
+ * sourmash_b200.h -- C ABI of libsourmash_b200.so, the H100 (sm_90a) implementation of
  * sourmash's two data-parallel hot paths (FracMinHash sketching, sorted-u64 intersection).
  *
  * The library is a drop-in for the subset of the reference's C ABI
- * (/root/reference/include/sourmash.h, generated from src/core/src/ffi/ *.rs) that the
+ * (sourmash/include/sourmash.h, generated from src/core/src/ffi/ *.rs) that the
  * Python object model binds for these paths, plus NEW batched entry points (smb_*) that
  * replace the reference's per-pair / per-record Python loops.  Part 1 keeps the reference's
  * names, argument order, ownership and error protocol; each group cites what it replaces.

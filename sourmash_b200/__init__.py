@@ -1,4 +1,4 @@
-"""sourmash_b200 -- B200-native FracMinHash sketching and sorted-hash intersection.
+"""sourmash_b200 -- H100-native FracMinHash sketching and sorted-hash intersection.
 
 Drop-in for the two hot paths of sourmash (DESIGN.md, include/sourmash_b200.h):
 

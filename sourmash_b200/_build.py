@@ -1,9 +1,9 @@
-"""Build recipe for libsourmash_b200.so (nvcc, sm_100a only).  Used by __graft_entry__.build().
+"""Build recipe for libsourmash_b200.so (nvcc, sm_90a only: H100).  Used by __graft_entry__.build().
 
 Staleness is decided by CONTENT: a sha256 over every source, every header and the compiler flags is
-stored next to the library (`libsourmash_b200.so.stamp`, git-ignored like the library, shipped to the GPU
-box with it).  File times do not survive the push to the GPU box, a hash does -- the prebuilt library is
-used there as it is instead of being recompiled in front of the first test."""
+stored next to the library (`libsourmash_b200.so.stamp`, git-ignored like the library).  File times do not
+survive a copy of the tree to another machine, a hash does -- a prebuilt library that matches its sources is
+used as it is instead of being recompiled in front of the first test."""
 import glob
 import hashlib
 import os
@@ -16,7 +16,7 @@ STAMP = LIB + ".stamp"
 SOURCES = ["capi.cu", "sketch_kernels.cu", "compare_kernels.cu", "ingest.cu"]
 PUBLIC_HEADER = os.path.join(HERE, "..", "include", "sourmash_b200.h")
 OBJ_DIR = os.path.join(CSRC, "build")                 # git-ignored; only the linked .so ships
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC"]
 LINK_LIBS = ["-lz", "-ldl"]
 

@@ -2,7 +2,7 @@
 
 The library reports failures through a thread-local (code, message) slot instead of return
 codes (include/sourmash_b200.h; same protocol as the reference's FFI, whose Python half is
-/root/reference/src/sourmash/utils.py:9-78).  ``rustcall`` wraps one call in
+sourmash/src/sourmash/utils.py:9-78).  ``rustcall`` wraps one call in
 clear-slot / call / poll-slot / raise; ``RustObject`` owns an opaque handle and frees it with
 the class's ``__dealloc_func__``.  The names are kept so code written against the reference's
 helpers keeps working.

@@ -1,6 +1,6 @@
 """cffi ABI-mode binding of libsourmash_b200.so -- the same mechanism the reference uses
 for its Rust cdylib (maturin ``bindings = "cffi"`` generates ``sourmash/_lowlevel`` which
-dlopen()s the library; /root/reference/pyproject.toml:138-155, src/sourmash/utils.py:3).
+dlopen()s the library; sourmash/pyproject.toml:138-155, src/sourmash/utils.py:3).
 
 Exports ``ffi`` and ``lib`` like the reference's ``sourmash._lowlevel``.  The library must
 have been built (``python -m sourmash_b200._build`` / ``__graft_entry__.build()``); there is

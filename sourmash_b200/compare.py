@@ -1,6 +1,6 @@
 """All-vs-all comparison of signatures on the GPU.
 
-Function-for-function replacement of /root/reference/src/sourmash/compare.py (:14-358): the
+Function-for-function replacement of sourmash/src/sourmash/compare.py (:14-358): the
 reference walks ``itertools.combinations`` in Python and crosses the FFI three times per
 pair; here a list of signatures becomes one CSR SketchSet in HBM and one batched call
 produces the whole count matrix.  Float post-processing follows the reference's operation

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the sm_100a kernels of sourmash_b200.
+// common.cuh -- shared device/host helpers for the sm_90a kernels of sourmash_b200.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -10,8 +10,8 @@ typedef uint8_t u8;
 
 #define SMB_U64_MAX 0xffffffffffffffffULL
 
-// Number of SMs on a B200; grids for persistent-style kernels are sized in multiples of it.
-#define SMB_B200_SMS 148
+// Number of SMs on an H100 SXM; grids for persistent-style kernels are sized in multiples of it.
+#define SMB_SMS 132
 
 // Shared memory of kernels that tests/host_emul/simt.h also runs on the CPU (SMB_SIMT_EMUL: one CTA at a
 // time as cooperative fibers, so block-shared storage is plain static storage there).

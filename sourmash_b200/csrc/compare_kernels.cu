@@ -1,4 +1,4 @@
-// compare_kernels.cu -- sorted-u64 hash-set intersection kernels for sm_100a.
+// compare_kernels.cu -- sorted-u64 hash-set intersection kernels for sm_90a (H100).
 //
 // Replaces the reference's per-pair CPU loops:
 //   count_common          src/core/src/sketch/minhash.rs:539-558 (+ Intersection :915-953)
@@ -8,7 +8,7 @@
 // driven in the reference by Python loops (src/sourmash/compare.py:14-187,
 // src/sourmash/index/__init__.py:115-170,777-909).
 //
-// Design (B200): integer/byte work, no tensor cores.  The hot kernel keeps TA "table" rows
+// Design: integer/byte work, no tensor cores.  The hot kernel keeps TA "table" rows
 // resident in shared memory as sorted keys + a bucket directory (bucket = key >> shift, the
 // keys are murmur outputs, i.e. uniform), and streams the other operand's rows through
 // registers with coalesced 8-byte loads: each streamed element costs one directory lookup
@@ -73,7 +73,7 @@ void launch_max_last(const u64* hA, const u64* offA, int nA, const u64* hB, cons
     int total = nA + nB;
     if (total <= 0) return;
     int blocks = (total + 255) / 256;
-    if (blocks > SMB_B200_SMS * 4) blocks = SMB_B200_SMS * 4;
+    if (blocks > SMB_SMS * 4) blocks = SMB_SMS * 4;
     max_last_kernel<<<blocks, 256, 0, s>>>(hA, offA, nA, hB, offB, nB, d_max); count_launches(1);
 }
 
@@ -136,7 +136,7 @@ void launch_pairwise_generic(const u64* hA, const u64* offA, int nA, const u64* 
     if (nA <= 0 || nB <= 0) return;
     u64 npairs = (u64)nA * (u64)nB;
     u64 blocks = (npairs + 7) / 8;
-    if (blocks > (u64)SMB_B200_SMS * 16) blocks = (u64)SMB_B200_SMS * 16;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
     pairwise_generic_kernel<<<(unsigned)blocks, 256, 0, s>>>(hA, offA, nA, hB, offB, nB, out, ldo,
                                                             symmetric ? 1 : 0, tiles.shard,
                                                             tiles.n_shards > 0 ? tiles.n_shards : 1); count_launches(1);
@@ -154,7 +154,7 @@ void launch_pairwise_num(const u64* hA, const u64* offA, int nA, const u64* hB, 
     if (nA <= 0 || nB <= 0) return;
     u64 npairs = (u64)nA * (u64)nB;
     u64 blocks = (npairs + 7) / 8;
-    if (blocks > (u64)SMB_B200_SMS * 16) blocks = (u64)SMB_B200_SMS * 16;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
     pairwise_num_kernel<<<(unsigned)blocks, 256, 0, s>>>(hA, offA, nA, hB, offB, nB, num, common,
                                                         usize, ldo, symmetric ? 1 : 0); count_launches(1);
 }
@@ -170,11 +170,11 @@ void launch_pairwise_num(const u64* hA, const u64* offA, int nA, const u64* hB, 
 void launch_pairwise_angular(const u64* h, const u64* ab, const u64* off, int n,
                              unsigned long long* d_sumsq, double* out, cudaStream_t s) {
     if (n <= 0) return;
-    int b1 = (n + 7) / 8; if (b1 > SMB_B200_SMS * 16) b1 = SMB_B200_SMS * 16;
+    int b1 = (n + 7) / 8; if (b1 > SMB_SMS * 16) b1 = SMB_SMS * 16;
     row_sumsq_kernel<<<b1, 256, 0, s>>>(ab, off, n, d_sumsq); count_launches(1);
     u64 npairs = (u64)n * (u64)n;
     u64 blocks = (npairs + 7) / 8;
-    if (blocks > (u64)SMB_B200_SMS * 16) blocks = (u64)SMB_B200_SMS * 16;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
     pairwise_angular_kernel<<<(unsigned)blocks, 256, 0, s>>>(h, ab, off, n, d_sumsq, out); count_launches(1);
 }
 
@@ -213,7 +213,7 @@ void launch_finalize_rows(const u32* common, size_t n, const u64* off, int n_row
 
 
 void launch_build_global_dir(const u64* q, u64 nq, int shift, u64 nb, u32* dir, cudaStream_t s) {
-    const u64 cap_blocks = (u64)SMB_B200_SMS * 32;
+    const u64 cap_blocks = (u64)SMB_SMS * 32;
     u64 b1 = (nb + 1 + 255) / 256; if (b1 > cap_blocks) b1 = cap_blocks;
     global_dir_fill_kernel<<<(unsigned)b1, 256, 0, s>>>(dir, nb + 1, DIR_UNSET); count_launches(1);
     if (nq) {
@@ -228,7 +228,7 @@ void launch_build_query_bitmap(const u64* q, u64 nq, int shift, int fine_log2,
                                u32* bitmap, cudaStream_t s) {
     if (nq == 0) return;
     u64 blocks = (nq + 255) / 256;
-    if (blocks > (u64)SMB_B200_SMS * 32) blocks = (u64)SMB_B200_SMS * 32;
+    if (blocks > (u64)SMB_SMS * 32) blocks = (u64)SMB_SMS * 32;
     build_query_bitmap_kernel<<<(unsigned)blocks, 256, 0, s>>>(q, nq, (u32)shift, fine_log2, bitmap); count_launches(1);
 }
 
@@ -238,7 +238,7 @@ void launch_one_vs_many_global(const u64* q, u64 nq, const u32* dir, int shift, 
                                const u64* offB, int nB, u32* out, cudaStream_t s) {
     if (nB <= 0) return;
     int blocks = (nB + 7) / 8;
-    if (blocks > SMB_B200_SMS * 16) blocks = SMB_B200_SMS * 16;
+    if (blocks > SMB_SMS * 16) blocks = SMB_SMS * 16;
     one_vs_many_global_kernel<<<blocks, 256, 0, s>>>(q, nq, dir, (u32)shift, nb, bitmap, fine_log2,
                                                      hB, offB, nB, out); count_launches(1);
 }
@@ -264,7 +264,7 @@ int range_major_parts(u64 T) {
     const char* e = getenv("SMB_RM_RANGES");              // tests: few ranges on small sets
     if (e && atoi(e) > 0) return atoi(e);
     // two CTAs per SM, a whole number of waves; fewer, larger parts for small sets
-    return T >= (32u << 20) ? SMB_B200_SMS * 10 : SMB_B200_SMS * 2;
+    return T >= (32u << 20) ? SMB_SMS * 10 : SMB_SMS * 2;
 }
 
 // *out stays null (with cudaSuccess) when the layout does not apply (positions must fit 32 bits)
@@ -285,8 +285,8 @@ cudaError_t range_major_build(const u64* h, const u64* off, int n, u64 T, u64 ma
     u32 *bounds = nullptr, *cnt = nullptr;
     if ((e = scratch.alloc((void**)&bounds, (cells + n) * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&cnt, (cells + 1) * sizeof(u32))) != cudaSuccess) return e;
-    rm_bounds_kernel<<<SMB_B200_SMS * 16, 256, 0, s>>>(h, off, n, rm->width, P, bounds);
-    const unsigned grid = (unsigned)std::min<u64>((cells + 256) / 256, (u64)SMB_B200_SMS * 32);
+    rm_bounds_kernel<<<SMB_SMS * 16, 256, 0, s>>>(h, off, n, rm->width, P, bounds);
+    const unsigned grid = (unsigned)std::min<u64>((cells + 256) / 256, (u64)SMB_SMS * 32);
     rm_counts_kernel<<<grid, 256, 0, s>>>(bounds, n, P, cnt);
     size_t scan_bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cnt, (u32*)rm->m_slice, (long long)(cells + 1), s);
@@ -296,7 +296,7 @@ cudaError_t range_major_build(const u64* h, const u64* off, int n, u64 T, u64 ma
     rm_scatter_kernel<<<grid, 256, 0, s>>>(h, off, bounds, (const u32*)rm->m_slice, n, P, (u64*)rm->m_rm);
     rm->nc = (n >> RM_COARSE_LOG2) + 2;
     if ((e = cudaMallocAsync(&rm->m_coarse, (size_t)P * rm->nc * sizeof(u32), s)) != cudaSuccess) return e;
-    rm_coarse_kernel<<<(unsigned)std::min<u64>(((u64)P * rm->nc + 255) / 256, (u64)SMB_B200_SMS * 32), 256, 0, s>>>(
+    rm_coarse_kernel<<<(unsigned)std::min<u64>(((u64)P * rm->nc + 255) / 256, (u64)SMB_SMS * 32), 256, 0, s>>>(
         (const u32*)rm->m_slice, n, P, rm->nc, (u32*)rm->m_coarse);
     count_launches(5);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
@@ -332,7 +332,7 @@ void launch_intersect_alive(const u64* q, u64 nq, const u8* alive, const u64* ro
 void launch_mark_dead(const u64* q, u64 nq, u8* alive, const u64* gone, u64 n, cudaStream_t s) {
     if (n == 0) return;
     u64 blocks = (n + 255) / 256;
-    if (blocks > (u64)SMB_B200_SMS * 8) blocks = (u64)SMB_B200_SMS * 8;
+    if (blocks > (u64)SMB_SMS * 8) blocks = (u64)SMB_SMS * 8;
     mark_dead_kernel<<<(unsigned)blocks, 256, 0, s>>>(q, nq, alive, gone, n); count_launches(1);
 }
 
@@ -416,7 +416,7 @@ static cudaError_t join_sort_slice(const u64* h, const u64* off, int n, u64 key_
     if ((e = cudaMallocAsync(&W.mem, Tp * (2 * sizeof(u64) + 2 * sizeof(u32)), s)) != cudaSuccess) return e;
     W.keys_a = (u64*)W.mem; W.keys_b = W.keys_a + Tp;
     W.ids_a = (u32*)(W.keys_b + Tp); W.ids_b = W.ids_a + Tp;
-    int blocks = n < SMB_B200_SMS * 16 ? n : SMB_B200_SMS * 16;
+    int blocks = n < SMB_SMS * 16 ? n : SMB_SMS * 16;
     join_gather_kernel<<<blocks, 256, 0, s>>>(h, off, d_beg, d_doff, n, W.keys_a, W.ids_a); count_launches(1);
     size_t sort_bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, W.keys_a, W.keys_b, W.ids_a, W.ids_b, (long long)T, 0, key_bits, s);
@@ -443,7 +443,7 @@ cudaError_t join_estimate(const u64* h, const u64* off, int n, u64 max_key, unsi
     cudaMemsetAsync(d_out2, 0, 2 * sizeof(unsigned long long), s);
     if (W.T) {
         u64 blocks = (W.T + 255) / 256;
-        if (blocks > (u64)SMB_B200_SMS * 32) blocks = (u64)SMB_B200_SMS * 32;
+        if (blocks > (u64)SMB_SMS * 32) blocks = (u64)SMB_SMS * 32;
         join_estimate_kernel<<<(unsigned)blocks, 256, 0, s>>>(W.keys_b, W.T, d_out2); count_launches(1);
     }
     cudaMemcpyAsync(r, d_out2, sizeof r, cudaMemcpyDeviceToHost, s);
@@ -583,11 +583,11 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     const u64 nblk = (T_all >> STRIPE_EBLK_LOG2) + 1;
     if ((e = scratch.alloc((void**)&eblk, (nblk + 1) * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&d_count, 16)) != cudaSuccess) return e;
-    const unsigned grid = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_B200_SMS * 32);
+    const unsigned grid = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_SMS * 32);
     const int low_bits = stripe_low_bits(max_key);
     // 1. 32-bit sort keys (top bits of the hashes) + payloads (low bits, element index)
     if (js->sharded) {
-        const int blocks = n < SMB_B200_SMS * 16 ? n : SMB_B200_SMS * 16;
+        const int blocks = n < SMB_SMS * 16 ? n : SMB_SMS * 16;
         stripe_keys_slice_kernel<<<blocks, 256, 0, s>>>(h, js->ebeg, d_doff, n, low_bits, key_a, pay_a);
     } else {
         stripe_keys_kernel<<<grid, 256, 0, s>>>(h, T, low_bits, key_a, pay_a);
@@ -606,13 +606,13 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     //    free: worklist) and redone in order, one warp per run (pay_a is free: the ordered payloads of those runs)
     u32* worklist = low_bits ? key_a : nullptr;
     if (low_bits) cudaMemsetAsync(d_count, 0, sizeof(u32), s);
-    stripe_eblk_kernel<<<(unsigned)std::min<u64>((nblk + 255) / 256, (u64)SMB_B200_SMS * 8), 256, 0, s>>>(off, n, T_all, eblk);
+    stripe_eblk_kernel<<<(unsigned)std::min<u64>((nblk + 255) / 256, (u64)SMB_SMS * 8), 256, 0, s>>>(off, n, T_all, eblk);
     if (js->tag16) stripe_tag_kernel<u16><<<grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u16*)js->tags, js->pos, worklist, d_count, js->swz);
     else stripe_tag_kernel<u32><<<grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u32*)js->tags, js->pos, worklist, d_count, js->swz);
     count_launches(2);
     if (low_bits) {
-        if (js->tag16) stripe_fix_kernel<u16><<<SMB_B200_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u16*)js->tags, js->pos, js->swz);
-        else stripe_fix_kernel<u32><<<SMB_B200_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz);
+        if (js->tag16) stripe_fix_kernel<u16><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u16*)js->tags, js->pos, js->swz);
+        else stripe_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz);
         count_launches(1);
     }
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
@@ -671,7 +671,7 @@ void launch_mirror_counts(void* d_counts, int bits, int n, cudaStream_t s) {
 }
 void launch_narrow_counts(const u32* in, u64 total, u16* out, cudaStream_t s) {
     if (!total) return;
-    stripe_narrow_counts_kernel<<<(unsigned)std::min<u64>((total + 255) / 256, (u64)SMB_B200_SMS * 32), 256, 0, s>>>(in, total, out);
+    stripe_narrow_counts_kernel<<<(unsigned)std::min<u64>((total + 255) / 256, (u64)SMB_SMS * 32), 256, 0, s>>>(in, total, out);
     count_launches(1);
 }
 
@@ -730,7 +730,7 @@ cudaError_t db_index_build(const u64* h, const u64* off, int n, u64 T, u64 max_k
     if ((e = scratch.alloc((void**)&keys_sorted, T * sizeof(u64))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&ids, T * sizeof(u32))) != cudaSuccess) return e;
     if ((e = cudaMallocAsync(&ix->m_rows, T * sizeof(u32), s)) != cudaSuccess) return e;
-    const int blocks = n < SMB_B200_SMS * 16 ? n : SMB_B200_SMS * 16;
+    const int blocks = n < SMB_SMS * 16 ? n : SMB_SMS * 16;
     index_rowid_kernel<<<blocks, 256, 0, s>>>(off, n, ids); count_launches(1);
     {   // (hash, row) pairs sorted by hash where they lie; stable, so rows ascend inside a group
         const int key_bits = key_bit_length(max_key);
@@ -785,14 +785,14 @@ u64 db_index_n_keys(const DbIndex* ix) { return ix->view.n_keys; }
 void launch_index_count(const DbIndex* ix, const u64* q, u64 nq, u32* counts, cudaStream_t s) {
     if (nq == 0 || ix->view.n_keys == 0) return;
     u64 blocks = (nq + 255) / 256;
-    if (blocks > (u64)SMB_B200_SMS * 16) blocks = (u64)SMB_B200_SMS * 16;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
     index_count_kernel<<<(unsigned)blocks, 256, 0, s>>>(ix->view, q, nq, nullptr, counts); count_launches(1);
 }
 // the same with the number of query hashes read from device memory (at most max_nq): no host round trip
 void launch_index_count_n(const DbIndex* ix, const u64* q, const u32* d_nq, u64 max_nq, u32* counts, cudaStream_t s) {
     if (max_nq == 0 || ix->view.n_keys == 0) return;
     u64 blocks = (max_nq + 255) / 256;
-    if (blocks > (u64)SMB_B200_SMS * 16) blocks = (u64)SMB_B200_SMS * 16;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
     index_count_kernel<<<(unsigned)blocks, 256, 0, s>>>(ix->view, q, max_nq, d_nq, counts); count_launches(1);
 }
 

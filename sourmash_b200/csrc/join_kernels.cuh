@@ -58,13 +58,11 @@ __global__ void __launch_bounds__(256) join_estimate_kernel(const u64* __restric
 
 // Every element pairs with the later elements of its group: ids ascend inside a group, so
 // (ids[p], ids[b]) is an upper-triangle cell.  Increments are fire-and-forget reductions (RED)
-// resolved in L2, and their rate is what bounds the kernel: 1.455e9 reductions in 16.7 ms =
-// 8.7e10 /s = 0.31 per clock per SM on the 10 000-sketch matrix, and three rewrites that attack
-// everything else left the time unchanged to 0.1 % (profiles/r1q_join.txt, r1s_join.txt):
-// evict-first stream loads + evict-last reductions (DRAM write-back 7.1 -> 1.4 GB, same time) and
-// walking the groups from a shared-memory tile instead of dependent L2 loads (long-scoreboard
-// stalls 105 -> 33 per issue, same time).  Going faster needs fewer reductions (accumulating in
-// shared-memory tiles of the matrix), see DESIGN.md section 4.5.
+// resolved in L2, and their rate is what bounds the kernel (1.44e9 reductions on the 10 000-sketch
+// matrix); rewrites that attack everything else -- evict-first stream loads + evict-last reductions,
+// walking the groups from a shared-memory tile instead of dependent L2 loads -- left the time
+// unchanged.  Going faster needs fewer reductions (accumulating in shared-memory tiles of the
+// matrix): the stripe layout of DESIGN.md section 4.5, the default.
 __global__ void __launch_bounds__(256) join_count_kernel(const u64* __restrict__ keys, const u32* __restrict__ ids,
                                                         u64 T, u32* __restrict__ common, size_t ld) {
     const u64 p = (u64)blockIdx.x * blockDim.x + threadIdx.x;

@@ -15,7 +15,7 @@
 //
 // The sorted stream is stored as
 //   tags[q] = row of sorted element q, top bit set on the first element of a group   (u16 if n < 32768: the
-//             whole stream of a 10 000 x 5 000 set is then 100 MB and stays in the 126 MB L2)
+//             whole stream of a 10 000 x 5 000 set is then 100 MB instead of 200 MB; each CTA reads it front to back)
 //   pos[e]  = sorted position of CSR element e
 // and is built with FOUR radix passes instead of seven: the sort key is the top 32 significant bits of the
 // hash, the remaining low bits travel in the 64-bit payload in front of the element index
@@ -421,8 +421,8 @@ __global__ void __launch_bounds__(256) stripe_finalize_counts_kernel(const Count
 }
 
 // out[i][j] = out[j][i] for i in [row_begin, row_end), j < i: 64 x 64 tiles through shared memory (four cells
-// per thread, so that a CTA has 32 KB of float64 in flight: with 32 x 32 tiles the kernel was bound by latency
-// at 2.4 TB/s), reads and writes both coalesced.  `full` points at row 0 of the whole matrix (rows < row_end
+// per thread, so that a CTA has 32 KB of float64 in flight: with 32 x 32 tiles the kernel was bound by latency),
+// reads and writes both coalesced.  `full` points at row 0 of the whole matrix (rows < row_end
 // are complete in their upper part).
 static constexpr int STRIPE_MIRROR_TILE = 64;
 template <typename T>

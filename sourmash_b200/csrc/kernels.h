@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers for the sm_100a kernels (internal C++ interface
+// kernels.h -- host-callable launchers for the sm_90a kernels (internal C++ interface
 // between capi.cu and the .cu kernel files; the public boundary is include/sourmash_b200.h).
 #pragma once
 #include <cuda_runtime.h>

@@ -93,7 +93,8 @@ __global__ void __launch_bounds__(HASH_THREADS) hash_kmers_kernel(HashArgs a) {
 // and 51 of `sourmash sketch dna`'s default parameter string in ONE pass over the bases -- one
 // rolling 51-state, the shorter k-mers read off it as prefixes -- instead of three launches that each
 // decode and roll the same bases.  Logic checked on the CPU by
-// tests/test_host_emulation.py::test_roll_fused_21_31_51_matches_oracle; measured 11.2 ms against 12.4 ms (profiles/r2a_ab.json).
+// tests/test_host_emulation.py::test_roll_fused_21_31_51_matches_oracle; on an H100 12.4 ms against 13.8 ms for the three
+// launches over 100 x 5 Mbp (bench.py --workload sketch, SMB_SKETCH_FUSED=0 for the second).
 // ---------------------------------------------------------------------------------------
 struct FusedArgs {
     HashArgs a;                   // row_index / max_hash unused

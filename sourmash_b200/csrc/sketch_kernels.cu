@@ -1,4 +1,4 @@
-// sketch_kernels.cu -- FracMinHash / MinHash sketch construction kernels for sm_100a.
+// sketch_kernels.cu -- FracMinHash / MinHash sketch construction kernels for sm_90a (H100).
 //
 // Replaces the reference's per-k-mer CPU loop:
 //   SeqToHashes::new / ::next (DNA branch)   src/core/src/signature.rs:190-232, 246-306
@@ -7,7 +7,7 @@
 //   SigsTrait::add_sequence                  src/core/src/signature.rs:38-58 (drop Ok(0))
 //   add_hash_with_abundance (scaled filter)  src/core/src/sketch/minhash.rs:313-383
 //
-// Design (B200): this path is integer-issue bound (~150 SASS integer ops per k-mer, 1 byte of
+// Design: this path is integer-issue bound (~150 SASS integer ops per k-mer, 1 byte of
 // HBM traffic per k-mer), so the kernel is organised around instruction count, not bytes:
 // every thread owns W consecutive windows and rolls the forward and reverse-complement
 // k-mers through registers as little-endian ASCII words (exactly the words murmur3 consumes)
@@ -139,9 +139,8 @@ void launch_hash_kmers_range(const HashLaunch& L, uint32_t ksize, int row_index,
     launch_hash_one_k<false>(a, ksize, rolled, hi - lo, s);
 }
 
-// k = 21, 31, 51 requested together are hashed by the one-pass kernel (measured on B200, profiles/r2a_ab.json:
-// 11.2 ms vs 12.4 ms for the three launches over 100 x 5 Mbp, identical sketches); SMB_SKETCH_FUSED=0 keeps
-// the three launches for A/B runs.
+// k = 21, 31, 51 requested together are hashed by the one-pass kernel (one read of the bases instead of three,
+// identical sketches); SMB_SKETCH_FUSED=0 keeps the three launches for A/B runs.
 bool sketch_fused_enabled() {
     const char* e = getenv("SMB_SKETCH_FUSED");
     return !(e && e[0] == '0');
@@ -291,7 +290,7 @@ void launch_first_invalid(const u8* bases, u64 len, unsigned long long* d_pos, c
     cudaMemsetAsync(d_pos, 0xff, sizeof(unsigned long long), s);
     if (len == 0) return;
     u64 blocks = (len + 255) / 256;
-    if (blocks > (u64)SMB_B200_SMS * 8) blocks = (u64)SMB_B200_SMS * 8;
+    if (blocks > (u64)SMB_SMS * 8) blocks = (u64)SMB_SMS * 8;
     first_invalid_kernel<<<(unsigned)blocks, 256, 0, s>>>(bases, len, d_pos); count_launches(1);
 }
 

@@ -231,8 +231,8 @@ __global__ void __launch_bounds__(TILE_THREADS_MAX, 1) pairwise_tile_kernel(Tile
 }
 
 // ------------------------------------------------------------------------------------
-// Split-word variant of the tile kernel (rows < 32760 keys, i.e. everything that fits).  The v1 kernel above runs at
-// ~98 % of the SM's shared-memory wavefront rate (ncu), two LDS.64 per probe being the bulk.
+// Split-word variant of the tile kernel (rows < 32760 keys, i.e. everything that fits).  The v1 kernel above is bound
+// by the SM's shared-memory wavefront rate, two LDS.64 per probe being the bulk.
 // Here the table keeps the low and high 32-bit halves of the keys in separate arrays: the
 // fast path touches only the low words (two LDS.32, ~1/2 the wavefronts) and remembers, per
 // probe, where a low word matched; the high words are read only for those probes, inside a

@@ -1,7 +1,7 @@
 """Jaccard / containment -> evolutionary distance (ANI) estimators.
 
 Host-side post-processing of the GPU's integer counts (SURVEY §8 f4): same estimators, argument
-names, result classes and thresholds as /root/reference/src/sourmash/distance_utils.py (:17-407;
+names, result classes and thresholds as sourmash/src/sourmash/distance_utils.py (:17-407;
 equations of Hera, Pierce-Ward & Koslicki, doi:10.1101/2022.01.11.475870), evaluated in Python
 floats in the reference's operation order so that values agree to the last bit.  The only
 numerical libraries involved are the ones the reference calls (scipy ``brentq``, ``norm.ppf``,

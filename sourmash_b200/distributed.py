@@ -49,9 +49,8 @@ class ShardGather:
         starts = np.concatenate([[0], np.cumsum(self.n_hashes)])
         # Two ranks: every shard lands where it belongs in the gathered array -- the views of an all_gather with shards of
         # different sizes (NCCL: one grouped broadcast per rank straight into its view; no padding, no compaction copy).
-        # Measured (profiles/r2e_* vs r2i_*): that wins at N = 2 (compare step 5.55 -> 4.78 ms together with the 16-bit
-        # counters) and LOSES at N = 8 (3.21 -> 3.70 ms: eight broadcasts are no match for one all-gather of equal blocks
-        # through the switch), so from four ranks on the shards travel as padded equal blocks and are compacted locally.
+        # That suits two ranks; with more, N broadcasts are no match for one all-gather of equal blocks through the
+        # switch, so from four ranks on the shards travel as padded equal blocks and are compacted locally.
         self._views = [self.hashes[int(starts[r]):int(starts[r + 1])] for r in range(world)]
         self._uneven_ok = dist.get_backend() == "nccl" and world <= 2 and all(int(x) > 0 for x in self.n_hashes)
         if not self._uneven_ok:                           # >= 4 ranks / gloo (CPU tests) / an empty shard: padded blocks + compaction

@@ -1,5 +1,5 @@
 """Exception mapping for the C ABI error codes (mirrors the behaviour of
-/root/reference/src/sourmash/exceptions.py:58-75: codes 100 < c < 10000 raise ValueError)."""
+sourmash/src/sourmash/exceptions.py:58-75: codes 100 < c < 10000 raise ValueError)."""
 from ._lowlevel import lib
 
 

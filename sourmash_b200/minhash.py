@@ -1,7 +1,7 @@
 """MinHash / FrozenMinHash: the sketch object model over the C ABI.
 
 Same public surface and semantics as the reference's ``sourmash.minhash``
-(/root/reference/src/sourmash/minhash.py:162-1258) so that code written against
+(sourmash/src/sourmash/minhash.py:162-1258) so that code written against
 ``sourmash.MinHash`` runs unchanged; every method is a thin call into
 ``libsourmash_b200.so`` (include/sourmash_b200.h part 1), where hashing and intersections
 execute on the GPU.  Float formulas that the reference evaluates in Python

@@ -1,7 +1,7 @@
-"""`sourmash scripts` commands backed by the B200 paths -- the reference's plugin route.
+"""`sourmash scripts` commands backed by the GPU paths -- the reference's plugin route.
 
 sourmash discovers command-line extensions through the ``sourmash.cli_script`` entry-point
-group (/root/reference/src/sourmash/plugins.py:8-12,91-186: a class with ``command``,
+group (sourmash/src/sourmash/plugins.py:8-12,91-186: a class with ``command``,
 ``description``, ``__init__(subparser)`` and ``main(args)``; the branchwater plugin uses the same
 hook).  With this package installed next to sourmash (see the entry points in pyproject.toml):
 
@@ -69,7 +69,7 @@ def parse_param_string(text):
 
 class Command_B200Sketch(CommandLinePlugin):
     command = "b200sketch"
-    description = "sketch FASTA/FASTQ files (dna, protein or translated) on a B200 GPU"
+    description = "sketch FASTA/FASTQ files (dna, protein or translated) on a GPU"
 
     def __init__(self, p):
         super().__init__(p)
@@ -116,7 +116,7 @@ def _select_args(p):
 
 class Command_B200Compare(CommandLinePlugin):
     command = "b200compare"
-    description = "all-vs-all Jaccard comparison of .sig files on a B200 GPU"
+    description = "all-vs-all Jaccard comparison of .sig files on a GPU"
 
     def __init__(self, p):
         super().__init__(p)
@@ -259,7 +259,7 @@ def _load_query_and_db(args):
 
 class Command_B200Gather(CommandLinePlugin):
     command = "b200gather"
-    description = "min-set-cover of a query sketch by database sketches on a B200 GPU (gather CSV)"
+    description = "min-set-cover of a query sketch by database sketches on a GPU (gather CSV)"
 
     def __init__(self, p):
         super().__init__(p)
@@ -290,7 +290,7 @@ class Command_B200Gather(CommandLinePlugin):
 
 class Command_B200Prefetch(CommandLinePlugin):
     command = "b200prefetch"
-    description = "all database sketches overlapping a query by a threshold, on a B200 GPU (prefetch CSV)"
+    description = "all database sketches overlapping a query by a threshold, on a GPU (prefetch CSV)"
 
     def __init__(self, p):
         super().__init__(p)
@@ -321,7 +321,7 @@ class Command_B200Prefetch(CommandLinePlugin):
 
 class Command_B200Search(CommandLinePlugin):
     command = "b200search"
-    description = "search a query sketch against database sketches on a B200 GPU (search CSV)"
+    description = "search a query sketch against database sketches on a GPU (search CSV)"
 
     def __init__(self, p):
         super().__init__(p)

@@ -1,6 +1,6 @@
 """SourmashSignature: named container of sketches over the C ABI.
 
-Mirrors the part of /root/reference/src/sourmash/signature.py (:29-527) that sits on the
+Mirrors the part of sourmash/src/sourmash/signature.py (:29-527) that sits on the
 hot path: construction from a MinHash, ``add_sequence`` (every sketch of the signature sees
 the sequence), the comparison delegates, md5sum identity, and ``.sig`` JSON I/O through the
 library's native reader / writer (csrc/ingest.cu; format: signature.rs:401-445).

@@ -1,6 +1,6 @@
 """`sourmash sketch dna | protein | translate` driver on the batched GPU path.
 
-Counterpart of the record loop of /root/reference/src/sourmash/command_sketch.py:662-789
+Counterpart of the record loop of sourmash/src/sourmash/command_sketch.py:662-789
 (`_compute_individual`: screed record loop -> ``sig.add_sequence(seq, force=not check_sequence)``
 or ``sig.add_protein(seq)`` when ``input_is_protein``): the input files are read natively
 (``smb_records_read``: FASTA/FASTQ, plain or gzip, one thread per file, sequence bytes in

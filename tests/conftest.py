@@ -13,8 +13,8 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def _ensure_built():
-    """Compile libsourmash_b200.so if it is missing or stale (needs nvcc; the GPU box receives the
-    prebuilt file with the snapshot).  Loaded by path so the package is not imported first."""
+    """Compile libsourmash_b200.so if it is missing or stale (needs nvcc; without it a library that is
+    already there is used).  Loaded by path so the package is not imported first."""
     import importlib.util
     spec = importlib.util.spec_from_file_location("_smb_build", os.path.join(ROOT, "sourmash_b200", "_build.py"))
     mod = importlib.util.module_from_spec(spec)
@@ -28,8 +28,29 @@ def _ensure_built():
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     _ensure_built()
+
+
+_ECOLI = []
+
+
+def ecoli_k12_path():
+    """The E. coli K-12 genome as one .fna.gz: stored as two gzip members (files under 1 MB each), whose concatenation is
+    a valid gzip file; written once per session into a temporary directory that is removed when the session ends."""
+    if not _ECOLI:
+        import atexit
+        import shutil
+        import tempfile
+        tmp = tempfile.mkdtemp(prefix="smb_golden_")
+        atexit.register(shutil.rmtree, tmp, True)
+        path = os.path.join(tmp, "ecoli_k12.fna.gz")
+        with open(path, "wb") as out:
+            for part in ("ecoli_k12.part1.fna.gz", "ecoli_k12.part2.fna.gz"):
+                with open(os.path.join(GOLDEN, part), "rb") as fh:
+                    out.write(fh.read())
+        _ECOLI.append(path)
+    return _ECOLI[0]
 
 
 def read_fasta(path):
@@ -52,7 +73,10 @@ def read_fasta(path):
 
 @pytest.fixture(scope="session")
 def golden():
-    arrays = np.load(os.path.join(GOLDEN, "golden_arrays.npz"))
+    arrays = {}
+    for part in ("golden_arrays_1.npz", "golden_arrays_2.npz"):     # two archives: each file stays under 1 MB
+        with np.load(os.path.join(GOLDEN, part)) as z:
+            arrays.update({k: z[k] for k in z.files})
     with open(os.path.join(GOLDEN, "golden_meta.json")) as fh:
         meta = json.load(fh)
     return {"arrays": arrays, "meta": meta}
@@ -60,7 +84,7 @@ def golden():
 
 @pytest.fixture(scope="session")
 def ecoli_seq():
-    recs = read_fasta(os.path.join(GOLDEN, "ecoli_k12.fna.gz"))
+    recs = read_fasta(ecoli_k12_path())
     assert len(recs) == 1
     return recs[0][1]
 

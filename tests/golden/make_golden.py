@@ -1,14 +1,15 @@
 #!/usr/bin/env python
 """Generate the golden parity fixtures in this directory from the reference's own test data.
 
-Run once in the build container (needs /root/reference, which does not exist on the GPU box):
+Run once with the reference checkout (oracle/reference.py: BASELINE.json's reference_path, or SMB_REFERENCE):
 
-    python tests/golden/make_golden.py
+    SMB_REFERENCE=<checkout> python tests/golden/make_golden.py
 
 Outputs (committed):
-  golden_arrays.npz   uint64 hash arrays pulled verbatim out of the reference's .sig fixtures
+  golden_arrays_1.npz, golden_arrays_2.npz   uint64 hash arrays pulled verbatim out of the reference's .sig fixtures
   golden_meta.json    md5sums, parameters and known-answer values quoted from the reference tests
-  ecoli_k12.fna.gz    byte copy of data/GCF_000005845.2_ASM584v2_genomic.fna.gz (BASELINE config 1 input)
+  ecoli_k12.part1.fna.gz, ecoli_k12.part2.fna.gz   data/GCF_000005845.2_ASM584v2_genomic.fna.gz (BASELINE config 1
+                      input) as two gzip members, split at a line; their concatenation is the genome's .fna.gz
   genome-s10.fa.gz    byte copy of tests/test-data/genome-s10.fa.gz (multi-record FASTA, num=500 golden sig)
   ecoli.faa, ecoli.genes.fna   byte copies of the protein / gene inputs of the known-good protein tests
 
@@ -19,10 +20,14 @@ import gzip
 import json
 import os
 import shutil
+import sys
 
 import numpy as np
 
-REF = "/root/reference"
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from oracle.reference import checkout  # noqa: E402
+
+REF = checkout()
 TD = os.path.join(REF, "tests", "test-data")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -50,8 +55,12 @@ for rec, s in sketches(os.path.join(TD, "GCF_000005845.2_ASM584v2_genomic.fna.gz
     ecoli[str(k)] = {"md5sum": s["md5sum"], "max_hash": s["max_hash"], "seed": s["seed"],
                      "num": s["num"], "n": len(s["mins"])}
 meta["ecoli"] = ecoli
-shutil.copyfile(os.path.join(REF, "data", "GCF_000005845.2_ASM584v2_genomic.fna.gz"),
-                os.path.join(HERE, "ecoli_k12.fna.gz"))
+with gzip.open(os.path.join(REF, "data", "GCF_000005845.2_ASM584v2_genomic.fna.gz"), "rb") as fh:
+    lines = fh.read().split(b"\n")
+for i, part in enumerate((b"\n".join(lines[:len(lines) // 2]) + b"\n", b"\n".join(lines[len(lines) // 2:]))):
+    with open(os.path.join(HERE, "ecoli_k12.part%d.fna.gz" % (i + 1)), "wb") as fh:
+        with gzip.GzipFile(fileobj=fh, mode="wb", compresslevel=9, mtime=0, filename="") as g:
+            g.write(part)
 
 # --- 47.fa / 63.fa (k=31, scaled=1000): tests/test_prefetch.py:272, test_index_protocol.py:217-269
 for name in ("47", "63"):
@@ -174,7 +183,14 @@ meta["kat"] = {
     "translate_codon": {"TCT": "S", "TC": "S", "T": "X"},
 }
 
-np.savez_compressed(os.path.join(HERE, "golden_arrays.npz"), **arrays)
+names = sorted(arrays, key=lambda k: -arrays[k].nbytes)         # two archives of about equal size: each under 1 MB
+parts, sizes = ({}, {}), [0, 0]
+for k in names:
+    i = 0 if sizes[0] <= sizes[1] else 1
+    parts[i][k] = arrays[k]
+    sizes[i] += arrays[k].nbytes
+np.savez_compressed(os.path.join(HERE, "golden_arrays_1.npz"), **parts[0])
+np.savez_compressed(os.path.join(HERE, "golden_arrays_2.npz"), **parts[1])
 with open(os.path.join(HERE, "golden_meta.json"), "w") as fh:
     json.dump(meta, fh, indent=1)
 print("wrote", len(arrays), "arrays")

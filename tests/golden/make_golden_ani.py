@@ -2,11 +2,11 @@
 """Golden vectors for the ANI / distance estimators (SURVEY §8 f4).
 
 distance_utils.py of the reference is plain Python (scipy + numpy), so unlike the Rust core it CAN
-be executed in the build container: this script imports /root/reference/src/sourmash/
+be executed without a Rust toolchain: this script imports <checkout>/src/sourmash/
 distance_utils.py by path (with a stub for its `.logging` import; nothing else of the package is
 needed) and records its outputs on a grid of inputs.  The result is committed as
 golden_ani.json; tests/test_distance_utils.py compares sourmash_b200.distance_utils with it
-bit-for-bit.  Run once in the build container:  python tests/golden/make_golden_ani.py
+bit-for-bit.  Run once:  SMB_REFERENCE=<sourmash checkout> python tests/golden/make_golden_ani.py
 """
 import importlib.util
 import itertools
@@ -15,7 +15,10 @@ import os
 import sys
 import types
 
-REF = "/root/reference/src/sourmash"
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+from oracle.reference import checkout  # noqa: E402
+
+REF = os.path.join(checkout(), "src", "sourmash")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 pkg = types.ModuleType("refsourmash")

@@ -1,4 +1,4 @@
-"""Dry run of bench.py's B200 arm without a GPU: the emulated library plays the device, a stand-in for the few
+"""Dry run of bench.py's GPU arm without a GPU: the emulated library plays the device, a stand-in for the few
 torch.cuda calls bench.py makes supplies streams / events / "device" tensors (host memory), and the workloads are
 shrunk by patching bench's size constants from outside.  NOT a measurement -- it only proves that every code path of
 bench.py assembles its JSON line (keys, types) without raising, for each workload and switch.
@@ -63,7 +63,7 @@ torch.Tensor.pin_memory = lambda self, *a, **kw: self
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 import bench  # noqa: E402
 
-# tiny stand-ins for the two workload generators (the emulated device is ~10^4 x slower than a B200)
+# tiny stand-ins for the two workload generators (the emulated device is ~10^4 x slower than a GPU)
 import numpy as np  # noqa: E402
 
 from sourmash_b200.synth import synth_genome, synth_sketches  # noqa: E402
@@ -99,12 +99,12 @@ LINES = []
 bench.emit_json = lambda obj: LINES.append(json.loads(json.dumps(obj)))
 
 
-def run(workload, env=None, extra=(), cpu_baseline=False):
+def run(workload, env=None, extra=(), cpu_baseline=False, dump=False):
     old = {k: os.environ.get(k) for k in (env or {})}
     os.environ.update(env or {})
     try:
         args = types.SimpleNamespace(gpus=1, steps=1, warmup=3, impl="b200", workload=workload, no_cpu_baseline=not cpu_baseline,
-                                     index="--index" in extra)
+                                     index="--index" in extra, dump_outputs="dump" if dump else None)
         n0 = len(LINES)
         bench.run_b200(args)
         assert len(LINES) == n0 + 1, "one JSON line per run"
@@ -150,6 +150,24 @@ def main():
         assert "index" in indexed and indexed["index"]["distinct_hashes"] > 0 and "index" not in plain
         if workload == "gather":
             assert plain["rounds"] == ranged["rounds"] == indexed["rounds"] > 2, (plain["rounds"], ranged["rounds"], indexed["rounds"])
+    # --dump-outputs: the arrays of the last timed step, float64, the same on a second run of the same arguments
+    import tempfile
+    dumps = []
+    for _ in range(2):
+        bench.DUMP.clear()
+        for workload in ("both", "search", "gather"):
+            run(workload, dump=True)
+        with tempfile.TemporaryDirectory() as d:
+            bench.write_dump(d)
+            dumps.append({f[:-4]: np.load(os.path.join(d, f)) for f in sorted(os.listdir(d))})
+    assert set(dumps[0]) == {"compare_row_ids", "compare_jaccard_rows", "sketch_hashes_hi32", "sketch_hashes_lo32",
+                             "sketch_row_offsets", "search_counts", "gather_rows", "gather_intersections"}, sorted(dumps[0])
+    for name, a in dumps[0].items():
+        assert a.dtype == np.float64 and np.array_equal(a, dumps[1][name]), name
+    assert dumps[0]["compare_jaccard_rows"].shape == (160, 160) and len(dumps[0]["sketch_row_offsets"]) == 10
+    hashes = dumps[0]["sketch_hashes_hi32"].astype(np.uint64) << np.uint64(32) | dumps[0]["sketch_hashes_lo32"].astype(np.uint64)
+    off = dumps[0]["sketch_row_offsets"].astype(np.int64)
+    assert all((np.diff(hashes[off[i]:off[i + 1]].astype(np.float64)) >= 0).all() for i in range(9))
     print("bench dry run ok: %d JSON lines assembled" % len(LINES))
 
 

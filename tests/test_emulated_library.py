@@ -58,7 +58,7 @@ def test_emulated_sharded_search_and_gather_world2():
 
 
 def test_emulated_smoke_hook():
-    "__graft_entry__.smoke() -- the driver's GPU smoke test -- against the emulated library"
+    "__graft_entry__.smoke() -- the end-to-end GPU smoke run -- against the emulated library"
     code = ("import sys; sys.path.insert(0, %r); import emulated_boot; emulated_boot.install(); sys.path.insert(0, %r); "
             "import __graft_entry__ as g; g.smoke()") % (os.path.join(HERE, "host_emul"), os.path.dirname(HERE))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
@@ -67,9 +67,9 @@ def test_emulated_smoke_hook():
 
 @pytest.mark.timeout(900)
 def test_bench_b200_arm_dry_run():
-    """bench.py's B200 arm against the emulated library with tiny workloads and a stand-in for its torch.cuda calls:
+    """bench.py's GPU arm against the emulated library with tiny workloads and a stand-in for its torch.cuda calls:
     not a measurement, a proof that every workload / switch assembles its JSON line (roofline, dram, issue, e2e,
-    launches, clocks) without raising -- the driver's end-of-round bench must not die on a KeyError."""
+    launches, clocks) and its --dump-outputs arrays without raising -- a benchmark run must not die on a KeyError."""
     script = os.path.join(HERE, "host_emul", "bench_dryrun.py")
     r = subprocess.run([sys.executable, script], capture_output=True, text=True, timeout=800)
     assert r.returncode == 0 and "bench dry run ok" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]

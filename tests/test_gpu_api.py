@@ -390,8 +390,8 @@ def test_sketch_fasta_files_matches_golden_signatures(smb, golden):
     """`sourmash sketch dna` on the two reference genomes -> the reference's own .sig contents."""
     import os
     from sourmash_b200.sketch import read_sequences, sketch_fasta_files
-    from tests.conftest import GOLDEN
-    ecoli, s10 = os.path.join(GOLDEN, "ecoli_k12.fna.gz"), os.path.join(GOLDEN, "genome-s10.fa.gz")
+    from tests.conftest import GOLDEN, ecoli_k12_path
+    ecoli, s10 = ecoli_k12_path(), os.path.join(GOLDEN, "genome-s10.fa.gz")
     sigs = sketch_fasta_files([ecoli, s10], ksizes=[21, 31, 51], scaled=1000, name_from_first=True)
     assert len(sigs) == 2 and len(sigs[0]) == 3 and sigs[0].filename == ecoli
     assert sigs[0].name.startswith("NC_000913.3 Escherichia coli")

@@ -1,4 +1,4 @@
-"""Parity of the CUDA kernels (through the C ABI) against the CPU oracle.  Needs a B200."""
+"""Parity of the CUDA kernels (through the C ABI) against the CPU oracle.  Needs an H100."""
 import numpy as np
 import pytest
 

@@ -9,15 +9,16 @@ import numpy as np
 import pytest
 
 import oracle as orc
+from oracle import reference
 import sourmash_b200 as smb
 from sourmash_b200.sigset import SignatureSet
 from sourmash_b200.sketch import RecordBatch, read_sequences
 
-from tests.conftest import GOLDEN, read_fasta
+from tests.conftest import GOLDEN, ecoli_k12_path, read_fasta
 
 
 def test_fasta_reader_matches_python_reader():
-    paths = [os.path.join(GOLDEN, f) for f in ("genome-s10.fa.gz", "ecoli.faa", "ecoli.genes.fna", "ecoli_k12.fna.gz")]
+    paths = [os.path.join(GOLDEN, f) for f in ("genome-s10.fa.gz", "ecoli.faa", "ecoli.genes.fna")] + [ecoli_k12_path()]
     rb = RecordBatch(paths, n_threads=3)
     want = [(i, n, s) for i, p in enumerate(paths) for n, s in read_fasta(p)]
     assert len(rb) == len(want)
@@ -177,10 +178,13 @@ def test_gather_fixture_bruteforce_matches_reference_expectation(golden):
     assert got == golden["meta"]["gather_k21_expected"]
 
 
-REF_DATA = "/root/reference/tests/test-data"
+# the reference's signature corpus (7 MB of .sig files): from the copy build() makes (oracle/reference.py)
+REF_DATA = os.path.join(reference.root(), "tests", "test-data")
+# the reference's FASTA / FASTQ test files, stored as they are
+REF_SEQ_DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refdata")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_DATA), reason="reference checkout not present (build container only)")
+@pytest.mark.skipif(not os.path.isdir(REF_DATA), reason="needs the reference copy that build() makes from its checkout")
 def test_native_parser_on_the_reference_fixture_corpus():
     """Every .sig / .sig.gz the reference ships as test data (hundreds of files: old writers,
     abundances, protein / dayhoff / hp, num and scaled, multi-signature files) through the native
@@ -242,13 +246,12 @@ def _py_records(path):
     return out
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_DATA), reason="reference checkout not present (build container only)")
 def test_native_reader_on_the_reference_sequence_files():
     import glob
     paths = []
     for pat in ("*.fa", "*.fa.gz", "*.fna", "*.fna.gz", "*.faa", "*.faa.gz", "*.fq.gz", "*.fq", "*.fastq", "*.fasta"):
-        paths += glob.glob(os.path.join(REF_DATA, "**", pat), recursive=True)
-        paths += glob.glob(os.path.join(os.path.dirname(os.path.dirname(REF_DATA)), "data", pat))
+        paths += glob.glob(os.path.join(REF_SEQ_DATA, "**", pat), recursive=True)
+        paths += glob.glob(os.path.join(os.path.dirname(REF_SEQ_DATA), pat))
     paths = sorted(set(p for p in paths if os.path.getsize(p) > 0))
     assert len(paths) > 12
     checked = 0
@@ -358,7 +361,7 @@ def test_xz_and_zstd_inputs(tmp_path):
 def test_malformed_inputs_give_parse_errors_not_crashes():
     """tests/tools/fuzz_ingest.py for a few seconds with a fixed seed: mutated .sig / .zip / FASTA / FASTQ inputs, each batch
     parsed in a child process -- an exception through the ABI is fine, a signal or a hang is not (longer runs, also under
-    AddressSanitizer: profiles/r2q_cpu_side_checks.md)."""
+    AddressSanitizer: README.md)."""
     import subprocess
     import sys
     tool = os.path.join(os.path.dirname(os.path.abspath(__file__)), "tools", "fuzz_ingest.py")

@@ -9,13 +9,26 @@ next to it, and every plugin command is run next to the reference's own command 
     sourmash compare                            vs   sourmash scripts b200compare     -> equal matrix, labels, CSV
     sourmash search / gather / prefetch         vs   sourmash scripts b200search ...  -> byte-identical CSV files
 
-Both sides run on the emulated library (no GPU where the reference checkout is); the reference's commands go sketch by
-sketch and pair by pair through the C ABI, the plugin commands through this package's batched entry points."""
+Both sides run on the emulated library; the reference's commands go sketch by sketch and pair by pair through the C ABI,
+the plugin commands through this package's batched entry points.
+
+What the reference's commands write is stored in tests/golden/plugin_cli_reference.json.gz (paths of the inputs and of the
+work directory replaced by placeholders), so without the reference the test runs the plugin commands
+(`python -m sourmash_b200.plugin ...`) on the same inputs and compares them with the stored files.  With the reference
+copy that build() makes (oracle/reference.py) the reference's commands run live, through its plugin loader, and what
+they write must equal the stored files; SMB_PLUGIN_CLI_RECORD=1 rewrites the stored file instead."""
+import base64
 import csv
 import glob
+import gzip
+import io
+import json
 import os
+import shutil
 import subprocess
 import sys
+import zipfile
+import zlib
 
 import numpy as np
 import pytest
@@ -26,33 +39,85 @@ import test_reference_python_over_abi as over_abi  # noqa: E402
 REF = over_abi.REF
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-DATA = os.path.join(REF, "tests", "test-data")
-
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "src", "sourmash")),
-                                reason="needs the reference checkout (this container only)")
+GOLDEN = os.path.join(HERE, "golden")
+LIVE = os.path.isdir(os.path.join(REF, "src", "sourmash"))
+STORED = os.path.join(GOLDEN, "plugin_cli_reference.json.gz")
+DATA = os.path.join(REF, "tests", "test-data")        # without the reference: a copy of the inputs in the reference's layout
+DATA_FILES = (["genome-s10.fa.gz", "genome-s11.fa.gz", "genome-s12.fa.gz", "short.fa", "short2.fa", "short3.fa", "ecoli.faa",
+               "ecoli.genes.fna", "47.fa.sig", "63.fa.sig", "2.fa.sig", "track_abund/47.fa.sig", "track_abund/63.fa.sig",
+               "prot/protein/GCA_001593925.1_ASM159392v1_protein.faa.gz.sig",
+               "prot/protein/GCA_001593935.1_ASM159393v1_protein.faa.gz.sig", "gather/combined.sig"]
+              + ["gather/" + os.path.basename(p) for p in sorted(glob.glob(os.path.join(GOLDEN, "gather", "GCF*.sig")))])
 
 COMMANDS = ("B200Sketch", "B200Compare", "B200Search", "B200Gather", "B200Prefetch")
 
 
+def _stored_inputs(dest):
+    "the reference's input files of this module, from tests/golden (as they are, or gzipped under refdata/)"
+    for rel in DATA_FILES:
+        out = os.path.join(dest, rel)
+        os.makedirs(os.path.dirname(out), exist_ok=True)
+        for src in (os.path.join(GOLDEN, "refdata", rel), os.path.join(GOLDEN, rel)):
+            if os.path.exists(src):
+                shutil.copy(src, out)
+                break
+        else:
+            with gzip.open(os.path.join(GOLDEN, "refdata", rel + ".gz")) as fh, open(out, "wb") as o:
+                o.write(fh.read())
+
+
+def _comparable(rel, data):
+    """What must be equal between two runs of a reference command: the bytes, except for a .zip archive, which records
+    when it was written -- its members' names and contents (gzip members decompressed: their headers carry a time too)."""
+    if not rel.endswith(".zip"):
+        return data
+    with zipfile.ZipFile(io.BytesIO(data)) as z:
+        return sorted((i.filename, gzip.decompress(z.read(i)) if i.filename.endswith(".gz") else z.read(i))
+                      for i in z.infolist())
+
+
+def _files(work):
+    found = {}
+    for top, _dirs, names in os.walk(work):
+        for n in names:
+            path = os.path.join(top, n)
+            found[os.path.relpath(path, work)] = os.stat(path).st_mtime_ns
+    return found
+
+
 @pytest.fixture(scope="module")
 def cli(tmp_path_factory):
+    global DATA
     sys.path.insert(0, os.path.join(HERE, "host_emul"))
     try:
         import emul_lib
     finally:
         sys.path.pop(0)
     tmp = str(tmp_path_factory.mktemp("refcli"))
-    over_abi._stub_package(tmp, emul_lib.build())
     site = os.path.join(tmp, "site")
-    info = os.path.join(site, "sourmash_b200-0.1.0.dist-info")         # what `pip install .` writes from pyproject.toml
-    os.makedirs(info)
-    with open(os.path.join(info, "METADATA"), "w") as fh:
-        fh.write("Metadata-Version: 2.1\nName: sourmash_b200\nVersion: 0.1.0\n")
-    with open(os.path.join(ROOT, "pyproject.toml")) as fh:
-        declared = [line.split("=")[0].strip() for line in fh if "sourmash_b200.plugin:Command_" in line]
-    assert declared == [c.lower() for c in COMMANDS]                   # the entry points written below are the declared ones
-    with open(os.path.join(info, "entry_points.txt"), "w") as fh:
-        fh.write("[sourmash.cli_script]\n" + "".join("%s = sourmash_b200.plugin:Command_%s\n" % (c.lower(), c) for c in COMMANDS))
+    if LIVE:
+        over_abi._stub_package(tmp, emul_lib.build())
+        info = os.path.join(site, "sourmash_b200-0.1.0.dist-info")     # what `pip install .` writes from pyproject.toml
+        os.makedirs(info)
+        with open(os.path.join(info, "METADATA"), "w") as fh:
+            fh.write("Metadata-Version: 2.1\nName: sourmash_b200\nVersion: 0.1.0\n")
+        with open(os.path.join(ROOT, "pyproject.toml")) as fh:
+            declared = [line.split("=")[0].strip() for line in fh if "sourmash_b200.plugin:Command_" in line]
+        assert declared == [c.lower() for c in COMMANDS]               # the entry points written below are the declared ones
+        with open(os.path.join(info, "entry_points.txt"), "w") as fh:
+            fh.write("[sourmash.cli_script]\n" + "".join("%s = sourmash_b200.plugin:Command_%s\n" % (c.lower(), c) for c in COMMANDS))
+        recorded = {}
+        stored = {}
+        if os.path.exists(STORED) and not os.environ.get("SMB_PLUGIN_CLI_RECORD"):
+            with gzip.open(STORED, "rt") as fh:                         # what the live reference writes must match it
+                stored = json.load(fh)
+    else:
+        emul_lib.build()
+        os.makedirs(site)
+        DATA = os.path.join(tmp, "test-data")
+        _stored_inputs(DATA)
+        with gzip.open(STORED, "rt") as fh:
+            recorded = json.load(fh)
     with open(os.path.join(site, "sitecustomize.py"), "w") as fh:       # this package too binds the emulated library
         fh.write("import sys\nsys.path.insert(0, %r); sys.path.insert(0, %r)\nimport emulated_boot\nemulated_boot.install()\n"
                  % (os.path.join(HERE, "host_emul"), ROOT))
@@ -60,26 +125,61 @@ def cli(tmp_path_factory):
     work = os.path.join(tmp, "work")
     os.makedirs(work)
 
+    def placeholders(data):
+        return data.replace(work.encode(), b"@WORK@").replace(DATA.encode(), b"@DATA@")
+
+    def key(args):
+        return placeholders(json.dumps([str(a) for a in args]).encode()).decode()
+
     def run(*args, rc=(0,)):
-        r = subprocess.run([sys.executable, "-m", "sourmash"] + [str(a) for a in args], capture_output=True, text=True, env=env,
-                           cwd=work, timeout=900)
+        if args[0] == "scripts" and not LIVE:                           # the plugin commands without the reference's loader
+            cmd = [sys.executable, "-m", "sourmash_b200.plugin"] + [str(a) for a in args[1:]]
+        else:
+            cmd = [sys.executable, "-m", "sourmash"] + [str(a) for a in args]
+        if args[0] != "scripts" and not LIVE:                           # a reference command: what it wrote, from the stored file
+            assert key(args) in recorded, "no stored outputs of the reference for %s" % key(args)
+            for rel, text in recorded[key(args)].items():
+                data = base64.b64decode(text).replace(b"@WORK@", work.encode()).replace(b"@DATA@", DATA.encode())
+                os.makedirs(os.path.dirname(os.path.join(work, rel)), exist_ok=True)
+                with open(os.path.join(work, rel), "wb") as fh:
+                    fh.write(data)
+            return None
+        before = _files(work)
+        r = subprocess.run(cmd, capture_output=True, text=True, env=env, cwd=work, timeout=900)
         assert r.returncode in rc, " ".join(map(str, args)) + "\n" + r.stdout[-2000:] + r.stderr[-3000:]
+        if args[0] != "scripts":                                        # LIVE: keep what the reference's command wrote
+            after = _files(work)
+            out = {}
+            for rel in sorted(after):
+                if before.get(rel) != after[rel]:
+                    with open(os.path.join(work, rel), "rb") as fh:
+                        out[rel] = base64.b64encode(placeholders(fh.read())).decode()
+            recorded[key(args)] = out
+            if key(args) in stored:
+                assert sorted(stored[key(args)]) == sorted(out), "the reference wrote other files than the stored ones"
+                for rel, text in out.items():
+                    assert _comparable(rel, base64.b64decode(text)) == _comparable(rel, base64.b64decode(stored[key(args)][rel])), \
+                        "the reference's %s differs from the stored one (%s)" % (rel, key(args))
         return r
 
-    def load(path):                                                      # with the reference's own loader
-        code = ("import sourmash, sys, json\n"
+    def load(path):                                                      # with the reference's own loader (or this package's)
+        code = ("import %s as sourmash, sys, json\n"
                 "print(json.dumps(sorted([ss.name, ss.filename, ss.md5sum(), ss.minhash.ksize, ss.minhash.moltype, "
                 "ss.minhash.scaled, ss.minhash.num, int(ss.minhash.track_abundance), sorted(ss.minhash.hashes.items())] "
-                "for ss in sourmash.load_file_as_signatures(sys.argv[1]))))")
+                "for ss in sourmash.load_file_as_signatures(sys.argv[1]))))") % ("sourmash" if LIVE else "sourmash_b200")
         r = subprocess.run([sys.executable, "-c", code, path], capture_output=True, text=True, env=env, cwd=work, timeout=900)
         assert r.returncode == 0, r.stderr[-3000:]
         return r.stdout
 
     def together(*cmdlines):
-        "several command lines at once (each is a process that spends a second importing the reference package)"
+        "several command lines: the reference's one by one (what each writes is noted), then the plugin's at once"
         from concurrent.futures import ThreadPoolExecutor
-        with ThreadPoolExecutor(len(cmdlines)) as pool:
-            return list(pool.map(lambda c: run(*c), cmdlines))
+        for c in cmdlines:
+            if c[0] != "scripts":
+                run(*c)
+        plugin = [c for c in cmdlines if c[0] == "scripts"]
+        with ThreadPoolExecutor(max(1, len(plugin))) as pool:
+            return list(pool.map(lambda c: run(*c), plugin))
 
     def loads(*paths):
         from concurrent.futures import ThreadPoolExecutor
@@ -87,9 +187,13 @@ def cli(tmp_path_factory):
             return list(pool.map(load, paths))
 
     run.work, run.load, run.loads, run.together = work, load, loads, together
-    return run
+    yield run
+    if LIVE and os.environ.get("SMB_PLUGIN_CLI_RECORD"):
+        with gzip.GzipFile(STORED, "wb", mtime=0) as fh:
+            fh.write(json.dumps(recorded, sort_keys=True, indent=0).encode())
 
 
+@pytest.mark.skipif(not LIVE, reason="the reference's own plugin loader: needs the reference copy that build() makes (oracle/reference.py)")
 def test_the_reference_lists_the_plugin_commands(cli):
     r = cli("scripts", rc=(0, 1))                          # no command given: the list of commands, exit status 1
     out = r.stderr + r.stdout
@@ -106,7 +210,7 @@ def test_the_reference_lists_the_plugin_commands(cli):
 ])
 def test_sketch_commands_write_equal_signatures(cli, kind, params, files):
     paths = [os.path.join(DATA, f) for f in files]
-    tag = "%s_%s" % (kind, abs(hash(params)) % 10**6)
+    tag = "%s_%s" % (kind, zlib.crc32(params.encode()) % 10**6)
     extra, plugin_params = [], params
     if kind != "dna":
         moltype = "dayhoff" if "dayhoff" in params else "hp" if ",hp" in params else "protein"

@@ -1,8 +1,8 @@
-"""The reference's CounterGather conformance suite -- /root/reference/tests/test_index_protocol.py:712-1312, the 22
+"""The reference's CounterGather conformance suite -- sourmash/tests/test_index_protocol.py:712-1312, the 22
 `test_counter_*` functions, read from the reference at test time and run UNMODIFIED -- against this package's
 CounterGather / MinHash / SourmashSignature.
 
-No GPU here and no /root/reference on the GPU box: the functions run in a subprocess whose library is the emulated
+The functions run in a subprocess whose library is the emulated
 build (tests/host_emul/emul_lib.py: the product's capi.cu and kernels, the device played by the CPU), like
 tests/test_reference_python_over_abi.py.  The GPU counterparts with their own data are tests/test_gpu_counter_gather_port.py.
 What is supplied here: the names the reference module imports at its top (`sourmash.MinHash`, `sourmash.load_one_signature`,
@@ -14,11 +14,14 @@ import sys
 
 import pytest
 
-REF_TESTS = "/root/reference/tests/test_index_protocol.py"
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import reference as _reference  # noqa: E402
+
+REF_TESTS = os.path.join(_reference.root(), "tests", "test_index_protocol.py")
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_TESTS), reason="needs the reference checkout (this container only)")
+pytestmark = pytest.mark.skipif(not os.path.exists(REF_TESTS), reason="needs the reference copy that build() makes from its checkout (oracle/reference.py)")
 
 HEADER = '''
 import os, sys

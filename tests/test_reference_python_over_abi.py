@@ -1,8 +1,8 @@
 """The reference's OWN Python -- object model, index classes, search / gather helpers, command line -- over this
 library's C ABI (SURVEY 8b, INTEGRATION.md section 2).
 
-/root/reference/src/sourmash is loaded IN PLACE (symlinks, nothing is copied) as a package `sourmash` whose
-`_lowlevel` is a cffi ABI-mode binding built from the REFERENCE header /root/reference/include/sourmash.h --
+sourmash/src/sourmash is loaded IN PLACE (symlinks, nothing is copied) as a package `sourmash` whose
+`_lowlevel` is a cffi ABI-mode binding built from the REFERENCE header sourmash/include/sourmash.h --
 exactly what maturin generates for the Rust cdylib (pyproject.toml:138-155) -- but dlopen()s libsourmash_b200
 instead.  The reference's own test modules (unmodified, read in place with their conftest.py and test-data) are
 then run by pytest in a subprocess: the object model (test_minhash.py, test_jaccard.py, test__minhash_hypothesis.py,
@@ -11,7 +11,7 @@ classes (test_search.py, test_index.py, test_index_protocol.py, test_api.py, tes
 its command line (`sourmash sketch ...`: test_sourmash_sketch.py; the CLI is run in-process through the entry point
 of a dist-info written next to the package, as sourmash_tst_utils.runscript expects).
 
-No GPU here and no /root/reference on the GPU box, so the "device" is the emulated build of the library
+The "device" is the emulated build of the library, so the suites run without a GPU
 (tests/host_emul/emul_lib.py: the product's capi.cu host glue and kernels compiled for the CPU, kernel
 launches executed by the SIMT emulator).  What this proves is the BOUNDARY: every symbol, struct layout,
 ownership rule, error code and message the reference's Python touches on these paths.  The kernels' results on
@@ -30,12 +30,15 @@ import textwrap
 
 import pytest
 
-REF = "/root/reference"
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import reference as _reference  # noqa: E402
+
+REF = _reference.root()                  # the copy build() makes (oracle/reference.py); the suites below skip without one
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
 pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "src", "sourmash")),
-                                reason="needs the reference checkout (this container only)")
+                                reason="needs the reference copy that build() makes from its checkout (oracle/reference.py)")
 
 LOWLEVEL = '''
 """cffi ABI-mode binding generated from the REFERENCE header, loading libsourmash_b200 (emulated build)."""
@@ -51,7 +54,7 @@ lib = ffi.dlopen({lib!r})
 '''
 
 INIT = '''
-"""Package __init__: the imports of /root/reference/src/sourmash/__init__.py in its order (the modules import each other
+"""Package __init__: the imports of sourmash/src/sourmash/__init__.py in its order (the modules import each other
 in circles that only resolve in this order), without its deprecated wrapper functions."""
 from ._lowlevel import ffi, lib
 ffi.init_once(lib.sourmash_init, "init")
@@ -303,7 +306,7 @@ def _check(r, at_least):
 
 @pytest.mark.timeout(3600)
 def test_reference_minhash_tests_pass_over_this_abi(tmp_path):
-    """/root/reference/tests/test_minhash.py (199 test functions, 311 cases with its fixtures), unmodified."""
+    """sourmash/tests/test_minhash.py (199 test functions, 311 cases with its fixtures), unmodified."""
     mods = ["test_minhash.py"]
     _check(_run_reference_tests(tmp_path, mods, _deselect(mods)), 300)
 

@@ -25,7 +25,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
 pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "src", "sourmash")),
-                                reason="needs the reference checkout (this container only)")
+                                reason="needs the reference copy that build() makes from its checkout (oracle/reference.py)")
 
 ALIAS_INIT = textwrap.dedent('''
     """`sourmash` = sourmash_b200 on the emulated library"""

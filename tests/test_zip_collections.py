@@ -2,7 +2,7 @@
 the collection loader against the plain-file loader, and the ``ZipFileLinearIndex`` /
 ``CollectionManifest`` scenarios of the reference (tests/test_index.py:688-1064,
 tests/test_manifest.py) -- on archives built here from the golden fixtures, and on the reference's
-own archives when its checkout is present (build container only).  The one-vs-many kernel is
+own archives (stored under tests/golden/refdata).  The one-vs-many kernel is
 replaced by the oracle where a search is involved (GPU counterpart: tests/test_gpu_zip.py)."""
 import glob
 import gzip
@@ -24,9 +24,7 @@ from sourmash_b200.sigset import SignatureSet
 from tests.conftest import GOLDEN
 from tests.test_index_glue import _FakeSet, cpu_kernels  # noqa: F401  (fixture)
 
-REF_DATA = "/root/reference/tests/test-data"
-needs_reference = pytest.mark.skipif(not os.path.isdir(REF_DATA),
-                                     reason="reference checkout not present (build container only)")
+REF_DATA = os.path.join(GOLDEN, "refdata")            # the reference's .zip test archives (tests/test-data), stored as they are
 GATHER = sorted(glob.glob(os.path.join(GOLDEN, "gather", "GCF*.sig")))
 
 
@@ -342,9 +340,8 @@ def test_zipfile_search_matches_linear_index(zip_db, cpu_kernels, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------
-# the reference's own archives (build container only)
+# the reference's own archives
 # ---------------------------------------------------------------------------------------------
-@needs_reference
 def test_reference_archives_load_like_zipfile_and_json():
     import json
     paths = [p for p in glob.glob(os.path.join(REF_DATA, "**", "*.zip"), recursive=True)]
@@ -386,7 +383,6 @@ def test_reference_archives_load_like_zipfile_and_json():
     assert checked > 10
 
 
-@needs_reference
 @pytest.mark.parametrize("use_manifest", [True, False])
 def test_reference_all_zip_scenarios(use_manifest):                           # tests/test_index.py:821-927
     path = os.path.join(REF_DATA, "prot", "all.zip")

@@ -4,7 +4,7 @@ every variant is first checked for equality with the default path's result on th
 inputs, then timed with CUDA events.  The library reads its switches with getenv() at call time, so
 os.environ changes between runs take effect.
 
-    python tests/tools/ab_variants.py [compare] [sketch] [search] [gather] > gpurun_out/ab.json
+    python tests/tools/ab_variants.py [compare] [sketch] [search] [gather] > ab.json
 
 Not a bench line (bench.py is): a development tool for GPU sessions."""
 import json

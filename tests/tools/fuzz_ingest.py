@@ -21,7 +21,8 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-REFDATA = "/root/reference/tests/test-data"
+REFDATA = os.path.join(os.environ.get("SMB_REFERENCE") or os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(
+    os.path.abspath(__file__)))), "oracle", "_ref", "sourmash"), "tests", "test-data")
 
 CHILD = r'''
 import os, sys
