@@ -368,6 +368,29 @@ uintptr_t smb_gather_intersect(SmbGatherState *st, uint32_t row, uint64_t *out_h
 uintptr_t smb_gather_apply(SmbGatherState *st, const uint64_t *intersect, uintptr_t n);
 void smb_gather_end(SmbGatherState *st);
 
+/* multigather (src/sourmash/commands.py:1124-1386): the gather of many queries against one resident database.
+ * q_hashes / q_offsets: the queries as CSR (n_queries + 1 offsets), each sorted and unique.  Per query:
+ * thresholds[i] -- stop when the best remaining overlap is below it (at least 1; NULL: 1) -- and min_counts[i] --
+ * only rows sharing at least that many hashes with the query take part (NULL: 1).  At most max_rounds picks per
+ * query.  The rounds of all queries run together on the device, a fixed number of launches per round; an indexed
+ * set, or candidate rows too large for the shared-memory table, take the session loop query by query -- the
+ * results are the same.  Every query's result equals smb_gather's for that query alone.
+ *   rounds    number of picks of query `query`
+ *   picks     its picked rows, |row ∩ remaining query| and |row ∩ query| per round (arrays of rounds() entries;
+ *             any may be NULL)
+ *   consumed  for every hash of every query (q_offsets[n_queries] entries): the round that took it, UINT32_MAX if none
+ *   round_launches  kernel launches of the batched rounds (prefetch not included) */
+typedef struct SmbMultiGather SmbMultiGather;
+SmbMultiGather *smb_multigather(const uint64_t *q_hashes, const uint64_t *q_offsets, uintptr_t n_queries,
+                                const SmbSketchSet *db, const uint32_t *thresholds, const uint32_t *min_counts,
+                                uintptr_t max_rounds);
+uintptr_t smb_multigather_rounds(const SmbMultiGather *m, uintptr_t query);
+void smb_multigather_picks(const SmbMultiGather *m, uintptr_t query, uint32_t *rows, uint32_t *sizes,
+                           uint32_t *overlaps);
+void smb_multigather_consumed(const SmbMultiGather *m, uint32_t *consumed_round);
+uint64_t smb_multigather_round_launches(const SmbMultiGather *m);
+void smb_multigather_free(SmbMultiGather *m);
+
 /* ==========================================================================================
  * Part 3: native ingest (SURVEY §8 f1, f2) -- the data formats either side of the hot paths,
  * read without per-record Python so that they do not dominate end to end.

@@ -326,6 +326,50 @@ def gather(query, db, threshold=1, max_rounds=None):
     return ids[:n].copy(), sizes[:n].copy()
 
 
+def multigather(queries, db, thresholds=None, min_counts=None, max_rounds=None, stats=None):
+    """gather() of every query (sorted-unique u64 arrays) against the one resident ``db``, the rounds of all queries run
+    together on the device.  ``thresholds`` / ``min_counts``: one per query (or one for all; default 1), as gather()'s
+    threshold and the least overlap a row needs to take part at all.  Returns, per query, (rows, sizes, consumed_round):
+    the picks as gather() returns them, and for every query hash the round that took it (UINT32_MAX: none).
+    ``stats`` (a dict) receives the kernel launches of the batched rounds ("round_launches") and, per query, the
+    overlap of every picked row with the whole query ("overlaps")."""
+    qs = [_u64(q) for q in queries]
+    n = len(qs)
+    offs = np.zeros(n + 1, dtype=np.uint64)
+    if n:
+        offs[1:] = np.cumsum([len(q) for q in qs])
+    hashes = np.concatenate(qs) if n else np.zeros(0, np.uint64)
+
+    def per_query(v):
+        if v is None:
+            return None
+        a = np.broadcast_to(np.asarray(v, dtype=np.int64), (n,))
+        return np.ascontiguousarray(np.clip(a, 0, 0xffffffff), dtype=np.uint32)
+    thr, mc = per_query(thresholds), per_query(min_counts)
+    if max_rounds is None:
+        max_rounds = len(db)
+    m = rustcall(lib.smb_multigather, _ptr(hashes, "uint64_t *"), _ptr(offs, "uint64_t *"), n, db._ptr,
+                 _ptr(thr, "uint32_t *") if thr is not None else ffi.NULL,
+                 _ptr(mc, "uint32_t *") if mc is not None else ffi.NULL, int(max_rounds))
+    try:
+        consumed = np.zeros(len(hashes), dtype=np.uint32)
+        lib.smb_multigather_consumed(m, _ptr(consumed, "uint32_t *"))
+        out = []
+        for i in range(n):
+            k = int(rustcall(lib.smb_multigather_rounds, m, i))
+            rows, sizes, overlaps = (np.zeros(k, dtype=np.uint32) for _ in range(3))
+            rustcall(lib.smb_multigather_picks, m, i, _ptr(rows, "uint32_t *"), _ptr(sizes, "uint32_t *"),
+                     _ptr(overlaps, "uint32_t *"))
+            out.append((rows, sizes, consumed[int(offs[i]):int(offs[i + 1])]))
+            if stats is not None:
+                stats.setdefault("overlaps", []).append(overlaps)
+        if stats is not None:
+            stats["round_launches"] = int(lib.smb_multigather_round_launches(m))
+        return out
+    finally:
+        lib.smb_multigather_free(m)
+
+
 class GatherSession:
     """Step-wise gather over one (local) database: begin / peek / intersect / apply
     (smb_gather_* of the C ABI).  ``gather()`` above is this loop run inside the library;

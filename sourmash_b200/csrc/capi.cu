@@ -2500,6 +2500,274 @@ uintptr_t smb_gather(const uint64_t* query, uintptr_t n_query, const SmbSketchSe
     });
 }
 
+// ---- multigather: the gather rounds of many queries against one resident database (multigather_kernels.cuh)
+struct SmbMultiGather {
+    std::vector<uint64_t> pick_off;          // [Q+1] into rows / sizes
+    std::vector<uint32_t> rows, sizes;       // the picks of every query, query after query
+    std::vector<uint32_t> overlaps;          // |picked row ∩ query| (its first counter)
+    std::vector<uint32_t> consumed;          // [total query hashes]: round that took the hash, UINT32_MAX if none
+    uint64_t round_launches = 0;             // kernel launches of the batched rounds
+};
+
+}  // extern "C"
+namespace {
+
+// a call through the C ABI (which records its own error) whose error is raised again inside the caller's guard
+template <typename F>
+auto abi_call(F&& f) -> decltype(f()) {
+    t_has_error = false;
+    auto r = f();
+    if (t_has_error) { t_has_error = false; throw SmbError(t_error); }
+    return r;
+}
+
+// device bytes one group of queries may take (SMB_MULTIGATHER_GROUP_BYTES overrides; the results do not depend on the
+// grouping): the queries' hashes and consumed rounds, and the candidates, picks and intersections of the batched rounds
+size_t multigather_group_bytes() {
+    const char* e = getenv("SMB_MULTIGATHER_GROUP_BYTES");
+    const long long v = e ? atoll(e) : 0;
+    return v > 0 ? (size_t)v : ((size_t)1 << 30);
+}
+
+struct MgQuery {
+    const uint64_t* q = nullptr;
+    size_t nq = 0;
+    uint64_t q_begin = 0;                    // offset of the query in the caller's CSR
+    uint32_t threshold = 1, min_count = 1;
+    std::vector<uint32_t> cand, cand_counts; // candidate rows (ascending) and their first counters
+    uint64_t isect_cap = 0, pick_cap = 0;
+    std::vector<uint32_t> rows, sizes;
+};
+
+// one query through the session loop: an indexed set, or candidate rows too large for the shared-memory table
+void multigather_session(MgQuery& g, const SmbSketchSet* db, uint32_t* consumed) {
+    if (g.cand.empty() || g.pick_cap == 0) return;
+    std::unique_ptr<SmbSketchSet> sub;
+    const SmbSketchSet* gdb = db;
+    // rows below min_count must not enter the counters; below the threshold they can never be picked anyway
+    if (g.min_count > g.threshold && g.cand.size() < db->n_rows) {
+        sub.reset(abi_call([&] { return smb_sketchset_take_rows(db, g.cand.data(), g.cand.size()); }));
+        gdb = sub.get();
+    }
+    std::unique_ptr<SmbGatherState> st(abi_call([&] { return smb_gather_begin_min(g.q, g.nq, gdb, g.threshold); }));
+    std::vector<uint64_t> buf(std::max<uint64_t>(gdb->max_len, 1));
+    size_t remaining = g.nq;
+    for (uint32_t r = 0; r < g.pick_cap && remaining > 0; ++r) {
+        uint32_t best = 0, row = 0;
+        abi_call([&] { smb_gather_peek(st.get(), &best, &row); return 0; });
+        if (best == 0 || best < g.threshold) break;
+        const size_t k = abi_call([&] { return smb_gather_intersect(st.get(), row, buf.data()); });
+        for (size_t i = 0; i < k; ++i) consumed[std::lower_bound(g.q, g.q + g.nq, buf[i]) - g.q] = r;
+        g.rows.push_back(sub ? g.cand[row] : row);
+        g.sizes.push_back((uint32_t)k);
+        remaining = abi_call([&] { return smb_gather_apply(st.get(), buf.data(), k); });
+    }
+}
+
+// the batched rounds of queries whose candidate rows fit the shared-memory table; their hashes and consumed rounds
+// already sit on the device at (q_begin - base) of d_q / d_consumed
+uint64_t multigather_batched(std::vector<MgQuery*>& grp, const SmbSketchSet* db, const uint64_t* d_q, uint32_t* d_consumed,
+                             uint64_t base, cudaStream_t s) {
+    const size_t K = grp.size();
+    std::vector<uint64_t> q_begin(K), q_end(K), cand_off(K + 1, 0), pick_off(K + 1, 0), isect_off(K + 1, 0);
+    std::vector<uint32_t> thr(K), cta_start(K + 1, 0);
+    constexpr int COLS = 16;                                  // candidate rows per decrement CTA (one per warp)
+    uint64_t max_cap = 0, max_isect = 0, max_key = set_max_key(*db, s);
+    for (size_t k = 0; k < K; ++k) {
+        const MgQuery& g = *grp[k];
+        q_begin[k] = g.q_begin - base;
+        q_end[k] = q_begin[k] + g.nq;
+        cand_off[k + 1] = cand_off[k] + g.cand.size();
+        pick_off[k + 1] = pick_off[k] + g.pick_cap;
+        isect_off[k + 1] = isect_off[k] + g.isect_cap;
+        cta_start[k + 1] = cta_start[k] + (uint32_t)((g.cand.size() + COLS - 1) / COLS);
+        thr[k] = g.threshold;
+        max_cap = std::max(max_cap, g.pick_cap);
+        max_isect = std::max(max_isect, g.isect_cap);
+        max_key = std::max(max_key, g.q[g.nq - 1]);
+    }
+    std::vector<uint32_t> cand(cand_off[K]), counts(cand_off[K]);
+    for (size_t k = 0; k < K; ++k) {
+        std::copy(grp[k]->cand.begin(), grp[k]->cand.end(), cand.begin() + cand_off[k]);
+        std::copy(grp[k]->cand_counts.begin(), grp[k]->cand_counts.end(), counts.begin() + cand_off[k]);
+    }
+    // one split table per decrement CTA: the longest intersection, a directory of about four buckets per key
+    smb::PairwisePlan one = smb::plan_pairwise(max_isect, max_key, 1);
+    const size_t key_bytes = (size_t)(one.cap + 2) * 8;
+    const uint64_t max_entries = std::min<uint64_t>((227 * 1024 - key_bytes) / 2 - 2, 60000);
+    const uint64_t want_entries = std::min<uint64_t>(max_entries, std::max<uint64_t>(4096, 4 * max_isect));
+    int sh = 0;
+    while (sh < 63 && (max_key >> sh) >= want_entries) ++sh;
+    const int nb = (int)((max_key >> sh) + 1);
+    const size_t smem = key_bytes + ((size_t)nb + 2) * 2;
+
+    DevBuf<uint64_t> d_qb(K, s), d_qe(K, s), d_cand_off(K + 1, s), d_pick_off(K + 1, s),
+        d_isect(std::max<uint64_t>(isect_off[K], 1), s), d_isect_off(K + 1, s);
+    DevBuf<uint32_t> d_cand(cand.size(), s), d_counts(counts.size(), s), d_delta(counts.size(), s),
+        d_pick_rows(std::max<uint64_t>(pick_off[K], 1), s), d_pick_sizes(std::max<uint64_t>(pick_off[K], 1), s),
+        d_state(2 * K, s), d_live(1, s), d_thr(K, s), d_isect_n(K, s), d_cta(K + 1, s);
+    d_qb.upload(q_begin.data(), K); d_qe.upload(q_end.data(), K);
+    d_cand.upload(cand.data(), cand.size()); d_cand_off.upload(cand_off.data(), K + 1);
+    d_counts.upload(counts.data(), counts.size()); d_delta.zero();
+    d_pick_off.upload(pick_off.data(), K + 1); d_isect_off.upload(isect_off.data(), K + 1);
+    d_state.zero(); d_thr.upload(thr.data(), K); d_cta.upload(cta_start.data(), K + 1);
+    uint32_t live = (uint32_t)K;
+    d_live.upload(&live, 1);
+    smb::MultiGatherArgs a{d_q, d_qb.p, d_qe.p, d_cand.p, d_cand_off.p, d_counts.p, d_delta.p, d_pick_off.p, d_pick_rows.p,
+                           d_pick_sizes.p, d_state.p, d_live.p, d_thr.p, d_consumed, d_isect.p, d_isect_off.p, d_isect_n.p,
+                           db->d_hashes, db->d_off, d_cta.p, (int)K, COLS, sh, nb, one.cap + 2};
+    // rounds enqueued in batches, the live counter read once per batch; a query stops by itself at its cap
+    const uint64_t launches0 = smb::g_launches.load();
+    const uint32_t batch = 16;
+    for (uint64_t issued = 0; live && issued < max_cap + 1; issued += batch) {
+        for (uint32_t k = 0; k < batch; ++k) smb::launch_multi_gather_round(a, cta_start[K], smem, s);
+        CK(cudaGetLastError());
+        d_live.download(&live, 1);
+        sync(s);
+    }
+    const uint64_t launches = smb::g_launches.load() - launches0;
+    std::vector<uint32_t> state(2 * K), prow(pick_off[K]), psize(pick_off[K]);
+    d_state.download(state.data(), 2 * K);
+    d_pick_rows.download(prow.data(), pick_off[K]);
+    d_pick_sizes.download(psize.data(), pick_off[K]);
+    sync(s);
+    for (size_t k = 0; k < K; ++k) {
+        MgQuery& g = *grp[k];
+        const uint32_t n = state[2 * k];
+        g.rows.assign(prow.begin() + pick_off[k], prow.begin() + pick_off[k] + n);
+        g.sizes.assign(psize.begin() + pick_off[k], psize.begin() + pick_off[k] + n);
+    }
+    return launches;
+}
+
+// queries [i, j): hashes uploaded once, first counters (one_vs_many_dev picks the range-major, global-directory, tile
+// or index regime; one readback per query), then the batched rounds, the consumed rounds read back once, and the
+// queries that need the session loop
+void multigather_group(std::vector<MgQuery>& qs, size_t i, size_t j, const SmbSketchSet* db, uint64_t max_rounds,
+                       SmbMultiGather* m, cudaStream_t s) {
+    const uint64_t base = qs[i].q_begin, n = qs[j - 1].q_begin + qs[j - 1].nq - base;
+    const size_t nB = db->n_rows;
+    DevBuf<uint64_t> d_q(std::max<uint64_t>(n, 1), s);
+    DevBuf<uint32_t> d_consumed(std::max<uint64_t>(n, 1), s), d_cnt(nB, s);
+    d_q.upload(qs[i].q, n);
+    CK(cudaMemsetAsync(d_consumed.p, 0xff, std::max<uint64_t>(n, 1) * 4, s));
+    std::vector<uint32_t> cnt(nB);
+    for (size_t k = i; k < j; ++k) {
+        MgQuery& g = qs[k];
+        if (g.nq == 0) continue;
+        d_cnt.zero();
+        one_vs_many_dev(d_q.p + (g.q_begin - base), g.nq, *db, d_cnt.p, s);
+        d_cnt.download(cnt.data(), nB);
+        sync(s);
+        uint64_t longest = 0;
+        for (size_t r = 0; r < nB; ++r)
+            if (cnt[r] >= g.min_count) {
+                g.cand.push_back((uint32_t)r);
+                g.cand_counts.push_back(cnt[r]);
+                longest = std::max<uint64_t>(longest, db->h_off[r + 1] - db->h_off[r]);
+            }
+        g.isect_cap = std::min<uint64_t>(g.nq, longest);
+        g.pick_cap = std::min<uint64_t>(max_rounds, g.cand.size());
+    }
+    const uint64_t mk = set_max_key(*db, s);
+    std::vector<MgQuery*> batched, session;
+    for (size_t k = i; k < j; ++k) {
+        MgQuery& g = qs[k];
+        if (g.cand.empty() || g.pick_cap == 0) continue;
+        const smb::PairwisePlan p = smb::plan_pairwise(g.isect_cap, std::max(mk, g.q[g.nq - 1]), 1);
+        (db->index || p.tables_per_cta == 0 || p.cap >= 32760 ? session : batched).push_back(&g);
+    }
+    // the candidates, picks and intersections of one launch of the rounds stay within the budget
+    const size_t budget = multigather_group_bytes();
+    std::vector<MgQuery*> part;
+    size_t part_bytes = 0;
+    auto flush = [&] {
+        if (!part.empty()) m->round_launches += multigather_batched(part, db, d_q.p, d_consumed.p, base, s);
+        part.clear();
+        part_bytes = 0;
+    };
+    for (MgQuery* g : batched) {
+        const size_t bytes = g->isect_cap * 8 + g->cand.size() * 16 + g->pick_cap * 8 + 64;
+        if (!part.empty() && part_bytes + bytes > budget) flush();
+        part.push_back(g);
+        part_bytes += bytes;
+    }
+    flush();
+    d_consumed.download(m->consumed.data() + base, n);
+    sync(s);
+    for (MgQuery* g : session) multigather_session(*g, db, m->consumed.data() + g->q_begin);
+}
+
+}  // namespace
+extern "C" {
+
+SmbMultiGather* smb_multigather(const uint64_t* q_hashes, const uint64_t* q_offsets, uintptr_t n_queries,
+                                const SmbSketchSet* db, const uint32_t* thresholds, const uint32_t* min_counts,
+                                uintptr_t max_rounds) {
+    return guarded<SmbMultiGather*>([&]() -> SmbMultiGather* {
+        cudaStream_t s = need_gpu();
+        const size_t Q = n_queries;
+        if (Q && q_offsets[0] != 0) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must start at 0");
+        std::vector<MgQuery> qs(Q);
+        for (size_t i = 0; i < Q; ++i) {
+            if (q_offsets[i + 1] < q_offsets[i]) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must not decrease");
+            MgQuery& g = qs[i];
+            g.q_begin = q_offsets[i];
+            g.q = q_hashes + g.q_begin;
+            g.nq = q_offsets[i + 1] - g.q_begin;
+            for (size_t j = 1; j < g.nq; ++j)
+                if (g.q[j] <= g.q[j - 1]) fail(SOURMASH_ERROR_CODE_MSG, "every query must be sorted and unique");
+            g.threshold = std::max<uint32_t>(thresholds ? thresholds[i] : 1, 1);
+            g.min_count = std::max<uint32_t>(min_counts ? min_counts[i] : 1, 1);
+        }
+        auto m = std::make_unique<SmbMultiGather>();
+        m->consumed.assign(Q ? q_offsets[Q] : 0, UINT32_MAX);
+        if (db->n_rows && max_rounds) {
+            // groups of consecutive queries: 12 bytes per query hash on the device, the rest of the budget for the rounds
+            const size_t budget = multigather_group_bytes();
+            for (size_t i = 0, j; i < Q; i = j) {
+                size_t bytes = qs[i].nq * 12;
+                for (j = i + 1; j < Q && bytes + qs[j].nq * 12 <= budget / 2; ++j) bytes += qs[j].nq * 12;
+                multigather_group(qs, i, j, db, max_rounds, m.get(), s);
+            }
+        }
+        m->pick_off.assign(Q + 1, 0);
+        for (size_t i = 0; i < Q; ++i) {
+            m->pick_off[i + 1] = m->pick_off[i] + qs[i].rows.size();
+            m->rows.insert(m->rows.end(), qs[i].rows.begin(), qs[i].rows.end());
+            m->sizes.insert(m->sizes.end(), qs[i].sizes.begin(), qs[i].sizes.end());
+            for (uint32_t r : qs[i].rows)
+                m->overlaps.push_back(qs[i].cand_counts[std::lower_bound(qs[i].cand.begin(), qs[i].cand.end(), r) - qs[i].cand.begin()]);
+        }
+        return m.release();
+    });
+}
+
+uintptr_t smb_multigather_rounds(const SmbMultiGather* m, uintptr_t query) {
+    return guarded<uintptr_t>([&]() -> uintptr_t {
+        if (query + 1 >= m->pick_off.size()) fail(SOURMASH_ERROR_CODE_MSG, "query index out of range");
+        return m->pick_off[query + 1] - m->pick_off[query];
+    });
+}
+
+void smb_multigather_picks(const SmbMultiGather* m, uintptr_t query, uint32_t* rows, uint32_t* sizes, uint32_t* overlaps) {
+    guarded_void([&] {
+        if (query + 1 >= m->pick_off.size()) fail(SOURMASH_ERROR_CODE_MSG, "query index out of range");
+        const uint64_t b = m->pick_off[query], e = m->pick_off[query + 1];
+        if (rows) std::copy(m->rows.begin() + b, m->rows.begin() + e, rows);
+        if (sizes) std::copy(m->sizes.begin() + b, m->sizes.begin() + e, sizes);
+        if (overlaps) std::copy(m->overlaps.begin() + b, m->overlaps.begin() + e, overlaps);
+    });
+}
+
+void smb_multigather_consumed(const SmbMultiGather* m, uint32_t* consumed_round) {
+    std::copy(m->consumed.begin(), m->consumed.end(), consumed_round);
+}
+
+uint64_t smb_multigather_round_launches(const SmbMultiGather* m) { return m->round_launches; }
+
+void smb_multigather_free(SmbMultiGather* m) { delete m; }
+
 // ==========================================================================================
 // Part 3: native ingest (csrc/ingest.cu) -- sequence files and .sig JSON without per-record Python
 // ==========================================================================================

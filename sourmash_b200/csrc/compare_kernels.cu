@@ -35,6 +35,7 @@
 #include "db_index.cuh"
 #include "db_index_kernels.cuh"
 #include "search_kernels.cuh"
+#include "multigather_kernels.cuh"
 #include "tile_kernels.cuh"
 #include "pair_kernels.cuh"
 
@@ -350,6 +351,15 @@ void launch_make_row_offsets(const u32* d_n, u64* d_off2, cudaStream_t s) {
 
 void launch_mark_dead_n(const u64* q, u64 nq, u8* alive, const u64* gone, const u32* d_n, cudaStream_t s) {
     mark_dead_n_kernel<<<64, 256, 0, s>>>(q, nq, alive, gone, d_n); count_launches(1);
+}
+
+void launch_multi_gather_round(const MultiGatherArgs& a, u32 cta_total, size_t smem_bytes, cudaStream_t s) {
+    if (a.n_queries <= 0) return;
+    multi_counter_update_argmax_pick_kernel<<<a.n_queries, 1024, 0, s>>>(a); count_launches(1);
+    multi_intersect_alive_pick_kernel<<<a.n_queries, 1024, 0, s>>>(a); count_launches(1);
+    if (cta_total == 0) return;
+    cudaFuncSetAttribute(multi_decrement_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    multi_decrement_kernel<<<cta_total, 512, smem_bytes, s>>>(a); count_launches(1);
 }
 
 void launch_intersect_rows(const u64* a, u64 na, const u64* b, u64 nb, u64* out, u32* d_n,

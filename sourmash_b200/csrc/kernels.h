@@ -157,6 +157,30 @@ void launch_intersect_alive_pick(const uint64_t* q, uint64_t nq, uint8_t* alive,
 void launch_mark_dead_n(const uint64_t* q, uint64_t nq, uint8_t* alive, const uint64_t* gone,
                         const uint32_t* d_n, cudaStream_t s);
 
+// gather rounds of many queries at once (multigather_kernels.cuh): per-query state in segments, three launches per round
+// for all queries.  The decrement launch runs cta_total CTAs with smem_bytes of dynamic shared memory (one split table
+// of kstride keys and nb + 2 directory entries).
+#ifndef SMB_MULTI_GATHER_ARGS_DEFINED
+#define SMB_MULTI_GATHER_ARGS_DEFINED
+struct MultiGatherArgs {
+    const uint64_t* q_hashes;
+    const uint64_t* q_begin;   const uint64_t* q_end;
+    const uint32_t* cand_rows; const uint64_t* cand_off;
+    uint32_t* counts;          uint32_t* delta;
+    const uint64_t* pick_off;  uint32_t* pick_rows; uint32_t* pick_sizes;
+    uint32_t* state;
+    uint32_t* live;
+    const uint32_t* threshold;
+    uint32_t* consumed;
+    uint64_t* isect;           const uint64_t* isect_off;
+    uint32_t* isect_n;
+    const uint64_t* db_hashes; const uint64_t* db_off;
+    const uint32_t* cta_start;
+    int n_queries, cols_per_cta, shift, nb, kstride;
+};
+#endif
+void launch_multi_gather_round(const MultiGatherArgs& a, uint32_t cta_total, size_t smem_bytes, cudaStream_t s);
+
 // Materialise A ∩ B of two sorted rows (gather's intersect_mh); returns count in *d_n.
 void launch_intersect_rows(const uint64_t* a, uint64_t na, const uint64_t* b, uint64_t nb,
                            uint64_t* out, uint32_t* d_n, cudaStream_t s);

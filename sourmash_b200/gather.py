@@ -93,22 +93,33 @@ def _size_ok(n, scaled, cache):
     return cache[key]
 
 
-def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, estimate_ani_ci=False,
-                     names=None, md5s=None, filenames=None, query_name="", query_filename="", max_rounds=None,
-                     noident_hashes=None, locations=None, query_orig=None):
-    """Min-set-cover of ``query_mh`` by the rows of the GPU-resident SketchSet ``db`` (same ksize,
-    seed and scaled as the query; use ``SketchSet.downsample`` / ``SignatureSet.to_sketchset``).
-    Returns the list of GatherRow in pick order -- the reference's GatherDatabases loop with the
-    columns of GatherResult.gatherresultdict.
+@dataclass
+class _GatherQuery:
+    "One query of a gather, prepared the way GatherDatabases.__init__ prepares it (search.py:803-818)."
+    mh: object
+    q_hashes: np.ndarray               # the query that is searched (noident hashes taken out), ascending
+    q_abunds: np.ndarray               # their abundances (ones when abundance is not tracked)
+    track: bool
+    noident_len: int
+    noident_weight: int
+    orig_len: int                      # orig_query_len, search.py:912
+    total_weighted: int
+    query_md5: str
+    query_bp_scaled: int
+    min_count: int                     # least overlap of a row that takes part at all
+    query_name: str
+    query_filename: str
+    q_size_ok: bool
+    cache: dict
 
-    ``noident_hashes``: hashes of the query known to match nothing (what ``sourmash gather`` collects
-    from its prefetch stage, commands.py:894-922,973): they are taken out of the query that is searched,
-    but stay in the denominators -- query_bp, query_n_hashes, f_orig_query, f_unique_to_query,
-    total_weighted_hashes -- and in remaining_bp (GatherDatabases.__init__ / __next__,
-    search.py:803-818,910-944; GatherResult.build_gather_result, search.py:553-590)."""
+
+def _prepare_query(query_mh, *, threshold_bp, ignore_abundance, noident_hashes, query_orig, query_name,
+                   query_filename):
+    """The searched query of a gather and everything its report columns need; None when no round can run (empty query,
+    or a threshold the query as given cannot reach)."""
     if not query_mh.scaled:
         raise TypeError("query signature must be calculated with scaled")
-    scaled, ksize = query_mh.scaled, query_mh.ksize
+    scaled = query_mh.scaled
     q_hashes = query_mh._mins_array()
     track = bool(query_mh.track_abundance) and not ignore_abundance
     q_abunds = query_mh._abunds_array() if track else np.ones(len(q_hashes), dtype=np.uint64)
@@ -124,22 +135,15 @@ def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, es
         noident_weight = int(q_abunds[gone].sum(dtype=object)) if track else noident_len
         q_hashes, q_abunds = q_hashes[~gone], q_abunds[~gone]
     search_len = len(q_hashes)
-    orig_len = search_len + noident_len                       # orig_query_len, search.py:912
-    rows = []
-    if search_len == 0 or len(db) == 0:
-        return rows
+    if search_len == 0:
+        return None
+    orig_len = search_len + noident_len
     total_weighted = (int(q_abunds.sum(dtype=object)) if track else search_len) + noident_weight
     # query_orig = (number of hashes, scaled, md5sum) of the query AS GIVEN, when ``query_mh`` is a downsampled copy of it: the
     # reference reports the given query's md5 and multiplies the hash count (at the comparison's scaled) by the GIVEN scaled
     # for query_bp (GatherResult.build_gather_result, search.py:553-561; BaseResult.get_cmpinfo, :222-243)
     query_md5 = (query_orig[2] if query_orig else query_mh.md5sum())[:8]
     query_bp_scaled = int(query_orig[1]) if query_orig else scaled
-    sizes = db.sizes()
-    counts0 = B.one_vs_many(q_hashes, db)                     # |match ∩ original query| for every row
-    cache = {}
-    q_size_ok = _size_ok(orig_len, scaled, cache)
-    alive = np.ones(search_len, dtype=bool)                    # hashes of the searched query not yet covered
-    remaining = search_len
     # which rows enter the rounds at all: the reference fills its counters by a prefetch of the query as given
     # (commands.py:906-911 -> CounterGather via Index.counter_gather); later rounds only ask count >= n_threshold_hashes
     min_count = 1
@@ -147,11 +151,90 @@ def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, es
         try:                                                   # unattainable for the query as given: no database yields a counter
             calc_threshold_from_bp(threshold_bp, int(query_orig[1]), int(query_orig[0]))      # (commands.py:909-914)
         except ValueError:
-            return rows
+            return None
         min_count = _min_count_of_given_query(threshold_bp, query_orig, orig_len)
+    cache = {}
+    return _GatherQuery(query_mh, q_hashes, q_abunds, track, noident_len, noident_weight, orig_len, total_weighted,
+                        query_md5, query_bp_scaled, min_count, query_name, query_filename, _size_ok(orig_len, scaled, cache),
+                        cache)
+
+
+def _gather_row(p, r, rank, ab, remaining, left_weight, c0, m, *, estimate_ani_ci, names, md5s, filenames, locations):
+    """The GatherResult columns of round ``rank`` (search.py:548-620): row ``r`` (``m`` hashes, ``c0`` shared with the
+    searched query) took the hashes whose abundances are ``ab`` (ascending hash order) from ``remaining`` live hashes;
+    ``left_weight`` is the weight of the live hashes after the round.  Python floats, the reference's operation order."""
+    mh = p.mh
+    scaled, ksize = mh.scaled, mh.ksize
+    u = len(ab)
+    g = GatherRow(row=int(r), gather_result_rank=rank, ksize=ksize, moltype=mh.moltype,
+                  scaled=scaled, query_name=p.query_name, query_filename=p.query_filename, query_md5=p.query_md5,
+                  query_bp=p.orig_len * p.query_bp_scaled, query_n_hashes=p.orig_len, total_weighted_hashes=p.total_weighted)
+    g.name = names[r] if names is not None else None
+    g.md5 = md5s[r] if md5s is not None else None
+    # the location the match was loaded from wins, else the filename stored in the match (search.py:230-235)
+    g.filename = locations[r] if locations is not None else (filenames[r] if filenames is not None else None)
+    g.intersect_bp = c0 * scaled
+    g.unique_intersect_bp = u * scaled
+    g.f_orig_query = c0 / p.orig_len
+    g.f_unique_to_query = u / p.orig_len
+    g.f_match_orig = _contained_by(c0, m, scaled)              # match.contained_by(original query)
+    g.f_match = _contained_by(u, m, scaled)                    # match.contained_by(remaining query)
+    g.remaining_bp = (p.noident_len + remaining - u) * scaled
+    if p.track:
+        g.query_abundance = True
+        g.n_unique_weighted_found = int(ab.sum(dtype=object))
+        g.f_unique_weighted = g.n_unique_weighted_found / p.total_weighted
+        vals = ab.tolist()
+        g.average_abund, g.median_abund, g.std_abund = np.mean(vals), np.median(vals), np.std(vals)
+    else:
+        g.f_unique_weighted = g.f_unique_to_query
+    g.sum_weighted_found = p.total_weighted - p.noident_weight - left_weight
+    # ANI columns: FracMinHashComparison(original query, match) (search.py:389-420, sketchcomparison.py:162-236)
+    ok = p.q_size_ok and _size_ok(m, scaled, p.cache)
+    qc = DU.containment_to_distance(_contained_by(c0, p.orig_len, scaled), ksize, scaled,
+                                    n_unique_kmers=p.orig_len * scaled, estimate_ci=estimate_ani_ci)
+    mc = DU.containment_to_distance(g.f_match_orig, ksize, scaled, n_unique_kmers=m * scaled,
+                                    estimate_ci=estimate_ani_ci)
+    qc.size_is_inaccurate = mc.size_is_inaccurate = not ok
+    g.query_containment_ani, g.match_containment_ani = qc.ani, mc.ani
+    g.potential_false_negative = bool(qc.p_exceeds_threshold or mc.p_exceeds_threshold)
+    if estimate_ani_ci:
+        g.query_containment_ani_low, g.query_containment_ani_high = qc.ani_low, qc.ani_high
+        g.match_containment_ani_low, g.match_containment_ani_high = mc.ani_low, mc.ani_high
+    if qc.ani is not None and mc.ani is not None:
+        g.average_containment_ani = (qc.ani + mc.ani) / 2
+        g.max_containment_ani = max(qc.ani, mc.ani)
+    return g
+
+
+def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, estimate_ani_ci=False,
+                     names=None, md5s=None, filenames=None, query_name="", query_filename="", max_rounds=None,
+                     noident_hashes=None, locations=None, query_orig=None):
+    """Min-set-cover of ``query_mh`` by the rows of the GPU-resident SketchSet ``db`` (same ksize,
+    seed and scaled as the query; use ``SketchSet.downsample`` / ``SignatureSet.to_sketchset``).
+    Returns the list of GatherRow in pick order -- the reference's GatherDatabases loop with the
+    columns of GatherResult.gatherresultdict.
+
+    ``noident_hashes``: hashes of the query known to match nothing (what ``sourmash gather`` collects
+    from its prefetch stage, commands.py:894-922,973): they are taken out of the query that is searched,
+    but stay in the denominators -- query_bp, query_n_hashes, f_orig_query, f_unique_to_query,
+    total_weighted_hashes -- and in remaining_bp (GatherDatabases.__init__ / __next__,
+    search.py:803-818,910-944; GatherResult.build_gather_result, search.py:553-590)."""
+    p = _prepare_query(query_mh, threshold_bp=threshold_bp, ignore_abundance=ignore_abundance,
+                       noident_hashes=noident_hashes, query_orig=query_orig, query_name=query_name,
+                       query_filename=query_filename)
+    rows = []
+    if p is None or len(db) == 0:
+        return rows
+    scaled = query_mh.scaled
+    q_hashes, q_abunds = p.q_hashes, p.q_abunds
+    sizes = db.sizes()
+    counts0 = B.one_vs_many(q_hashes, db)                     # |match ∩ original query| for every row
+    alive = np.ones(len(q_hashes), dtype=bool)                 # hashes of the searched query not yet covered
+    remaining = len(q_hashes)
     rowmap = None
-    if min_count > 1:                                          # the session's min_count is a hint; the rule is enforced here
-        rowmap = np.nonzero(counts0.astype(np.int64) >= min_count)[0].astype(np.uint32)
+    if p.min_count > 1:                                        # the session's min_count is a hint; the rule is enforced here
+        rowmap = np.nonzero(counts0.astype(np.int64) >= p.min_count)[0].astype(np.uint32)
         if len(rowmap) == 0:
             return rows
         sess = B.GatherSession(q_hashes, db.take_rows(rowmap), min_count=1)
@@ -170,53 +253,76 @@ def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, es
         isect = sess.intersect(r)                              # remaining query ∩ row r (ascending)
         if rowmap is not None:
             r = int(rowmap[r])                                 # row of the caller's database
-        u, m, c0 = len(isect), int(sizes[r]), int(counts0[r])
         pos = np.searchsorted(q_hashes, isect)
-        ab = q_abunds[pos]
         alive[pos] = False
         left = sess.apply(isect)
-        g = GatherRow(row=int(r), gather_result_rank=len(rows), ksize=ksize, moltype=query_mh.moltype,
-                      scaled=scaled, query_name=query_name, query_filename=query_filename, query_md5=query_md5,
-                      query_bp=orig_len * query_bp_scaled, query_n_hashes=orig_len, total_weighted_hashes=total_weighted)
-        g.name = names[r] if names is not None else None
-        g.md5 = md5s[r] if md5s is not None else None
-        # the location the match was loaded from wins, else the filename stored in the match (search.py:230-235)
-        g.filename = locations[r] if locations is not None else (filenames[r] if filenames is not None else None)
-        g.intersect_bp = c0 * scaled
-        g.unique_intersect_bp = u * scaled
-        g.f_orig_query = c0 / orig_len
-        g.f_unique_to_query = u / orig_len
-        g.f_match_orig = _contained_by(c0, m, scaled)          # match.contained_by(original query)
-        g.f_match = _contained_by(u, m, scaled)                # match.contained_by(remaining query)
-        g.remaining_bp = (noident_len + remaining - u) * scaled
-        if track:
-            g.query_abundance = True
-            g.n_unique_weighted_found = int(ab.sum(dtype=object))
-            g.f_unique_weighted = g.n_unique_weighted_found / total_weighted
-            vals = ab.tolist()
-            g.average_abund, g.median_abund, g.std_abund = np.mean(vals), np.median(vals), np.std(vals)
-        else:
-            g.f_unique_weighted = g.f_unique_to_query
-        g.sum_weighted_found = total_weighted - noident_weight - \
-            (int(q_abunds[alive].sum(dtype=object)) if track else int(alive.sum()))
-        # ANI columns: FracMinHashComparison(original query, match) (search.py:389-420, sketchcomparison.py:162-236)
-        ok = q_size_ok and _size_ok(m, scaled, cache)
-        qc = DU.containment_to_distance(_contained_by(c0, orig_len, scaled), ksize, scaled,
-                                        n_unique_kmers=orig_len * scaled, estimate_ci=estimate_ani_ci)
-        mc = DU.containment_to_distance(g.f_match_orig, ksize, scaled, n_unique_kmers=m * scaled,
-                                        estimate_ci=estimate_ani_ci)
-        qc.size_is_inaccurate = mc.size_is_inaccurate = not ok
-        g.query_containment_ani, g.match_containment_ani = qc.ani, mc.ani
-        g.potential_false_negative = bool(qc.p_exceeds_threshold or mc.p_exceeds_threshold)
-        if estimate_ani_ci:
-            g.query_containment_ani_low, g.query_containment_ani_high = qc.ani_low, qc.ani_high
-            g.match_containment_ani_low, g.match_containment_ani_high = mc.ani_low, mc.ani_high
-        if qc.ani is not None and mc.ani is not None:
-            g.average_containment_ani = (qc.ani + mc.ani) / 2
-            g.max_containment_ani = max(qc.ani, mc.ani)
-        rows.append(g)
+        left_weight = int(q_abunds[alive].sum(dtype=object)) if p.track else int(alive.sum())
+        rows.append(_gather_row(p, r, len(rows), q_abunds[pos], remaining, left_weight, int(counts0[r]), int(sizes[r]),
+                                estimate_ani_ci=estimate_ani_ci, names=names, md5s=md5s, filenames=filenames,
+                                locations=locations))
         remaining = left
     return rows
+
+
+def gather_many(query_mhs, db, *, threshold_bp=0, ignore_abundance=False, estimate_ani_ci=False, names=None, md5s=None,
+                filenames=None, locations=None, query_names=None, query_filenames=None, max_rounds=None,
+                noident_hashes=None, query_origs=None, db_scaled=None):
+    """gather_databases() of every query in ``query_mhs`` against the one resident ``db``; returns one list of GatherRow
+    per query, each equal to what gather_databases returns for that query alone.  The rounds of all queries at one
+    scaled run together on the device (batch.multigather); the report columns come from the picks, the overlaps and
+    the round that consumed each query hash, read back once.
+
+    ``db`` is sketched at ``db_scaled`` (default: the smallest scaled of the queries); queries at a coarser scaled are
+    compared with one downsampled copy of it per distinct scaled.  ``query_names``, ``query_filenames``,
+    ``noident_hashes`` and ``query_origs`` hold one entry per query (see gather_databases)."""
+    n = len(query_mhs)
+
+    def each(v, default=None):
+        return list(v) if v is not None else [default] * n
+    qnames, qfiles, noidents, origs = each(query_names, ""), each(query_filenames, ""), each(noident_hashes), each(query_origs)
+    out = [[] for _ in range(n)]
+    preps = [_prepare_query(mh, threshold_bp=threshold_bp, ignore_abundance=ignore_abundance, noident_hashes=noidents[i],
+                            query_orig=origs[i], query_name=qnames[i], query_filename=qfiles[i])
+             for i, mh in enumerate(query_mhs)]
+    by_scaled = {}
+    for i, p in enumerate(preps):
+        if p is None:
+            continue
+        try:                                                   # the first round's threshold check (search.py:15-37)
+            calc_threshold_from_bp(threshold_bp, p.mh.scaled, len(p.q_hashes))
+        except ValueError:
+            continue
+        by_scaled.setdefault(p.mh.scaled, []).append(i)
+    if not by_scaled or len(db) == 0:
+        return out
+    if db_scaled is None:
+        db_scaled = min(by_scaled)
+    for scaled in sorted(by_scaled):
+        if scaled < db_scaled:
+            raise ValueError("a query at scaled=%d cannot be compared with a database at scaled=%d" % (scaled, db_scaled))
+        sdb = db if scaled == db_scaled else db.downsample(B.max_hash_for_scaled(scaled))
+        idx = by_scaled[scaled]
+        # gather_databases' stop rule per round, best < threshold_bp / scaled, on integer counters
+        threshold = max(1, math.ceil(float(threshold_bp) / scaled)) if threshold_bp else 1
+        stats = {}
+        res = B.multigather([preps[i].q_hashes for i in idx], sdb, thresholds=threshold,
+                            min_counts=[preps[i].min_count for i in idx],
+                            max_rounds=len(sdb) if max_rounds is None else max_rounds, stats=stats)
+        sizes = sdb.sizes()
+        for i, (rows, _, consumed), overlaps in zip(idx, res, stats["overlaps"]):
+            p = preps[i]
+            order = np.argsort(consumed, kind="stable")        # hashes grouped by round, ascending inside each round
+            bounds = np.searchsorted(consumed[order], np.arange(len(rows) + 1, dtype=np.uint32))
+            remaining = len(p.q_hashes)
+            left_weight = int(p.q_abunds.sum(dtype=object)) if p.track else remaining
+            for k, r in enumerate(rows.tolist()):
+                ab = p.q_abunds[order[bounds[k]:bounds[k + 1]]]
+                left_weight -= int(ab.sum(dtype=object)) if p.track else len(ab)
+                out[i].append(_gather_row(p, r, k, ab, remaining, left_weight, int(overlaps[k]), int(sizes[r]),
+                                          estimate_ani_ci=estimate_ani_ci, names=names, md5s=md5s, filenames=filenames,
+                                          locations=locations))
+                remaining -= len(ab)
+    return out
 
 
 PREFETCH_COLUMNS = [  # search.py:364-388

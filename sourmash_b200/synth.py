@@ -146,3 +146,18 @@ def gather_workload(n_db, seed=5000, n_clusters=20, members=10, pool=6000, noise
             parts.append(v[rng.random(len(v)) < 0.6])
     parts.append(rng.integers(1, max_hash, size=noise, dtype=np.uint64, endpoint=True))
     return np.unique(np.concatenate(parts)), sizes, frac * 0.0, overrides
+
+
+def multigather_workload(n_db, n_queries, seed=5000):
+    """configs[4] for many samples: the queries of gather_workload under n_queries seeds and ONE database of n_db rows
+    holding the planted rows of all of them (a row planted by two queries keeps the content the later one gave it).
+    Returns (queries, sizes, frac (all zero), overrides {row: hashes}) for database_block."""
+    sizes, frac = database_plan(n_db, seed + 1)
+    queries, overrides = [], {}
+    for i in range(n_queries):
+        q, _, _, planted = gather_workload(n_db, seed=seed + 7919 * i)
+        queries.append(q)
+        for row, v in planted.items():
+            overrides[row] = v
+            sizes[row] = len(v)
+    return queries, sizes, frac * 0.0, overrides
