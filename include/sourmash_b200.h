@@ -342,6 +342,16 @@ void smb_one_vs_many(const uint64_t *query, uintptr_t n_query, const SmbSketchSe
 /* the same with the (sorted) query and the n_rows counters in device memory: nothing crosses PCIe */
 void smb_one_vs_many_dev(const uint64_t *d_query, uintptr_t n_query, const SmbSketchSet *db,
                          uint32_t *d_common_out);
+/* one_vs_many for many queries: counts_out[q * n_rows + r] = |query q ∩ row r| (a Q x n_rows host matrix).
+ * q_hashes / q_offsets: the queries as CSR (n_queries + 1 offsets from 0, not decreasing), each sorted and unique.
+ * Groups of consecutive queries share one streaming pass over the database (its range-major copy, built on first
+ * use); an indexed set, SMB_SEARCH_LAYOUT=global, or a group of one query counts query by query.  The counts are
+ * those of smb_one_vs_many for each query. */
+void smb_many_vs_many(const uint64_t *q_hashes, const uint64_t *q_offsets, uintptr_t n_queries,
+                      const SmbSketchSet *db, uint32_t *counts_out);
+/* the same with the hashes and the Q x n_rows counters in device memory; the offsets stay on the host */
+void smb_many_vs_many_dev(const uint64_t *d_q_hashes, const uint64_t *q_offsets, uintptr_t n_queries,
+                          const SmbSketchSet *db, uint32_t *d_counts_out);
 /* gather (CounterGather + GatherDatabases, src/sourmash/index/__init__.py:777-909,
  * src/sourmash/search.py:877-949): iterative min-set-cover.  Returns number of rounds;
  * match_ids/isect_sizes receive, per round, the chosen row and |match ∩ remaining query|.

@@ -314,6 +314,35 @@ def one_vs_many_device(d_query_ptr, n_query, db, d_counts_ptr):
              ffi.cast("uint32_t *", int(d_counts_ptr)))
 
 
+def _query_csr(queries):
+    "(hashes, offsets) of a list of sorted-unique u64 queries"
+    qs = [_u64(q) for q in queries]
+    offs = np.zeros(len(qs) + 1, dtype=np.uint64)
+    if qs:
+        offs[1:] = np.cumsum([len(q) for q in qs])
+    return (np.concatenate(qs) if qs else np.zeros(0, np.uint64)), offs
+
+
+def many_vs_many(queries, db):
+    """|query ∩ row| for every query (sorted-unique u64 arrays) and every row of ``db``: a (len(queries), len(db))
+    uint32 array equal to ``np.stack([one_vs_many(q, db) for q in queries])``.  Groups of queries share one pass over
+    the database on the device instead of one pass per query."""
+    hashes, offs = _query_csr(queries)
+    n = len(offs) - 1
+    out = np.zeros((n, len(db)), dtype=np.uint32)
+    rustcall(lib.smb_many_vs_many, _ptr(hashes, "uint64_t *"), _ptr(offs, "uint64_t *"), n, db._ptr,
+             _ptr(out, "uint32_t *"))
+    return out
+
+
+def many_vs_many_device(d_hashes_ptr, offsets, db, d_counts_ptr):
+    """many_vs_many with the queries' hashes and the (Q, len(db)) u32 counters in device memory; ``offsets`` (Q + 1,
+    host) delimit the queries inside the hashes."""
+    offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+    rustcall(lib.smb_many_vs_many_dev, ffi.cast("uint64_t *", int(d_hashes_ptr)), _ptr(offs, "uint64_t *"),
+             len(offs) - 1, db._ptr, ffi.cast("uint32_t *", int(d_counts_ptr)))
+
+
 def gather(query, db, threshold=1, max_rounds=None):
     """Iterative min-set-cover; returns (match_ids, intersect_sizes) in pick order."""
     q = _u64(query)
@@ -333,12 +362,8 @@ def multigather(queries, db, thresholds=None, min_counts=None, max_rounds=None, 
     the picks as gather() returns them, and for every query hash the round that took it (UINT32_MAX: none).
     ``stats`` (a dict) receives the kernel launches of the batched rounds ("round_launches") and, per query, the
     overlap of every picked row with the whole query ("overlaps")."""
-    qs = [_u64(q) for q in queries]
-    n = len(qs)
-    offs = np.zeros(n + 1, dtype=np.uint64)
-    if n:
-        offs[1:] = np.cumsum([len(q) for q in qs])
-    hashes = np.concatenate(qs) if n else np.zeros(0, np.uint64)
+    hashes, offs = _query_csr(queries)
+    n = len(offs) - 1
 
     def per_query(v):
         if v is None:

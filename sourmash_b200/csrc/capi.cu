@@ -2529,6 +2529,80 @@ size_t multigather_group_bytes() {
     return v > 0 ? (size_t)v : ((size_t)1 << 30);
 }
 
+// the checks of a query CSR (smb_multigather, smb_many_vs_many): hashes on the host, or null (checked on the device)
+void check_query_csr(const uint64_t* h, const uint64_t* off, size_t Q) {
+    if (Q && off[0] != 0) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must start at 0");
+    for (size_t i = 0; i < Q; ++i) {
+        if (off[i + 1] < off[i]) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must not decrease");
+        if (h)
+            for (uint64_t k = off[i] + 1; k < off[i + 1]; ++k)
+                if (h[k] <= h[k - 1]) fail(SOURMASH_ERROR_CODE_MSG, "every query must be sorted and unique");
+    }
+}
+
+// device bytes one group of many_vs_many may take: its G x n counters and 12 bytes per query hash (the merged key
+// stream and its query ids).  SMB_MANY_VS_MANY_GROUP_BYTES overrides; the counts do not depend on the grouping
+size_t many_vs_many_group_bytes() {
+    const char* e = getenv("SMB_MANY_VS_MANY_GROUP_BYTES");
+    const long long v = e ? atoll(e) : 0;
+    return v > 0 ? (size_t)v : ((size_t)1 << 30);
+}
+
+// How the counts of many queries against one set are made, chosen from the input alone: groups of two or more
+// consecutive queries share one range-major pass (the copy built on first use, as one_vs_many_dev builds it); a group
+// of one query, an indexed set, SMB_SEARCH_LAYOUT=global and a set the copy declines take one_vs_many_dev per query.
+struct MvmPlan {
+    const smb::RangeMajor* rm = nullptr;     // null: query by query
+    std::vector<size_t> cuts;                // group g = queries [cuts[g], cuts[g + 1])
+};
+
+// off: the Q + 1 offsets of the queries' CSR.  A group's counters and key stream stay within the byte budget, and its
+// keys within range_major_group_keys (sparse per-range bitmaps)
+MvmPlan many_vs_many_plan(const uint64_t* off, size_t Q, const SmbSketchSet& db, cudaStream_t s) {
+    MvmPlan p;
+    const size_t nB = db.n_rows;
+    if (Q >= 2 && nB && !db.index && smb::range_search_enabled()) {
+        if (!db.range_major && !db.range_major_tried) {
+            db.range_major_tried = true;
+            CK(smb::range_major_build(db.d_hashes, db.d_off, (int)nB, db.total(), set_max_key(db, s), &db.range_major, s));
+        }
+        p.rm = db.range_major;
+    }
+    const size_t budget = many_vs_many_group_bytes();
+    const uint64_t key_cap = p.rm ? smb::range_major_group_keys(p.rm) : UINT64_MAX;
+    p.cuts.push_back(0);
+    for (size_t i = 0, j; i < Q; i = j) {
+        uint64_t keys = off[i + 1] - off[i];
+        for (j = i + 1; j < Q; ++j) {
+            const uint64_t nk = off[j + 1] - off[j];
+            if ((j + 1 - i) * nB * 4 + (keys + nk) * 12 > budget || keys + nk > key_cap) break;
+            keys += nk;
+        }
+        p.cuts.push_back(j);
+    }
+    return p;
+}
+
+// counters of the plan's queries [a, b) into d_counts ((b - a) x n, query-major, zeroed by the caller); off: the CSR
+// offsets, the hashes of query a at d_q[0]
+void many_vs_many_group(const MvmPlan& p, const uint64_t* d_q, const uint64_t* off, size_t a, size_t b,
+                        const SmbSketchSet& db, uint32_t* d_counts, cudaStream_t s) {
+    const size_t nB = db.n_rows;
+    if (p.rm && b - a >= 2) {
+        std::vector<uint64_t> rel(b - a + 1);
+        for (size_t k = a; k <= b; ++k) rel[k - a] = off[k] - off[a];
+        DevBuf<uint64_t> d_off(rel.size(), s);
+        d_off.upload(rel.data(), rel.size());
+        bool unsorted = false;
+        CK(smb::many_vs_many_range_major(p.rm, d_q, d_off.p, (int)(b - a), rel.back(), d_counts, &unsorted, s));
+        sync(s);      // rel is a host temporary
+        if (unsorted) fail(SOURMASH_ERROR_CODE_MSG, "every query must be sorted and unique");
+        return;
+    }
+    for (size_t k = a; k < b; ++k)
+        one_vs_many_dev(d_q + (off[k] - off[a]), off[k + 1] - off[k], db, d_counts + (k - a) * nB, s);
+}
+
 struct MgQuery {
     const uint64_t* q = nullptr;
     size_t nq = 0;
@@ -2640,34 +2714,44 @@ uint64_t multigather_batched(std::vector<MgQuery*>& grp, const SmbSketchSet* db,
     return launches;
 }
 
-// queries [i, j): hashes uploaded once, first counters (one_vs_many_dev picks the range-major, global-directory, tile
-// or index regime; one readback per query), then the batched rounds, the consumed rounds read back once, and the
-// queries that need the session loop
+// queries [i, j): hashes uploaded once, first counters (the many-query pass of many_vs_many_group; one readback per
+// group of its plan), then the batched rounds, the consumed rounds read back once, and the queries that need the
+// session loop
 void multigather_group(std::vector<MgQuery>& qs, size_t i, size_t j, const SmbSketchSet* db, uint64_t max_rounds,
                        SmbMultiGather* m, cudaStream_t s) {
     const uint64_t base = qs[i].q_begin, n = qs[j - 1].q_begin + qs[j - 1].nq - base;
     const size_t nB = db->n_rows;
     DevBuf<uint64_t> d_q(std::max<uint64_t>(n, 1), s);
-    DevBuf<uint32_t> d_consumed(std::max<uint64_t>(n, 1), s), d_cnt(nB, s);
+    DevBuf<uint32_t> d_consumed(std::max<uint64_t>(n, 1), s);
     d_q.upload(qs[i].q, n);
     CK(cudaMemsetAsync(d_consumed.p, 0xff, std::max<uint64_t>(n, 1) * 4, s));
-    std::vector<uint32_t> cnt(nB);
-    for (size_t k = i; k < j; ++k) {
-        MgQuery& g = qs[k];
-        if (g.nq == 0) continue;
+    std::vector<uint64_t> off(j - i + 1);
+    for (size_t k = i; k < j; ++k) off[k - i] = qs[k].q_begin - base;
+    off[j - i] = n;
+    const MvmPlan plan = many_vs_many_plan(off.data(), j - i, *db, s);
+    std::vector<uint32_t> cnt;
+    for (size_t c = 0; c + 1 < plan.cuts.size(); ++c) {
+        const size_t a = plan.cuts[c], b = plan.cuts[c + 1];
+        DevBuf<uint32_t> d_cnt((b - a) * nB, s);
         d_cnt.zero();
-        one_vs_many_dev(d_q.p + (g.q_begin - base), g.nq, *db, d_cnt.p, s);
-        d_cnt.download(cnt.data(), nB);
+        many_vs_many_group(plan, d_q.p + off[a], off.data(), a, b, *db, d_cnt.p, s);
+        cnt.resize((b - a) * nB);
+        d_cnt.download(cnt.data(), cnt.size());
         sync(s);
-        uint64_t longest = 0;
-        for (size_t r = 0; r < nB; ++r)
-            if (cnt[r] >= g.min_count) {
-                g.cand.push_back((uint32_t)r);
-                g.cand_counts.push_back(cnt[r]);
-                longest = std::max<uint64_t>(longest, db->h_off[r + 1] - db->h_off[r]);
-            }
-        g.isect_cap = std::min<uint64_t>(g.nq, longest);
-        g.pick_cap = std::min<uint64_t>(max_rounds, g.cand.size());
+        for (size_t k = a; k < b; ++k) {
+            MgQuery& g = qs[i + k];
+            if (g.nq == 0) continue;
+            const uint32_t* row_cnt = cnt.data() + (k - a) * nB;
+            uint64_t longest = 0;
+            for (size_t r = 0; r < nB; ++r)
+                if (row_cnt[r] >= g.min_count) {
+                    g.cand.push_back((uint32_t)r);
+                    g.cand_counts.push_back(row_cnt[r]);
+                    longest = std::max<uint64_t>(longest, db->h_off[r + 1] - db->h_off[r]);
+                }
+            g.isect_cap = std::min<uint64_t>(g.nq, longest);
+            g.pick_cap = std::min<uint64_t>(max_rounds, g.cand.size());
+        }
     }
     const uint64_t mk = set_max_key(*db, s);
     std::vector<MgQuery*> batched, session;
@@ -2707,16 +2791,13 @@ SmbMultiGather* smb_multigather(const uint64_t* q_hashes, const uint64_t* q_offs
     return guarded<SmbMultiGather*>([&]() -> SmbMultiGather* {
         cudaStream_t s = need_gpu();
         const size_t Q = n_queries;
-        if (Q && q_offsets[0] != 0) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must start at 0");
+        check_query_csr(q_hashes, q_offsets, Q);
         std::vector<MgQuery> qs(Q);
         for (size_t i = 0; i < Q; ++i) {
-            if (q_offsets[i + 1] < q_offsets[i]) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must not decrease");
             MgQuery& g = qs[i];
             g.q_begin = q_offsets[i];
             g.q = q_hashes + g.q_begin;
             g.nq = q_offsets[i + 1] - g.q_begin;
-            for (size_t j = 1; j < g.nq; ++j)
-                if (g.q[j] <= g.q[j - 1]) fail(SOURMASH_ERROR_CODE_MSG, "every query must be sorted and unique");
             g.threshold = std::max<uint32_t>(thresholds ? thresholds[i] : 1, 1);
             g.min_count = std::max<uint32_t>(min_counts ? min_counts[i] : 1, 1);
         }
@@ -2740,6 +2821,61 @@ SmbMultiGather* smb_multigather(const uint64_t* q_hashes, const uint64_t* q_offs
                 m->overlaps.push_back(qs[i].cand_counts[std::lower_bound(qs[i].cand.begin(), qs[i].cand.end(), r) - qs[i].cand.begin()]);
         }
         return m.release();
+    });
+}
+
+// many_vs_many: the one-vs-many counts of many queries, groups of them sharing one pass over the database
+void smb_many_vs_many(const uint64_t* q_hashes, const uint64_t* q_offsets, uintptr_t n_queries, const SmbSketchSet* db,
+                      uint32_t* counts_out) {
+    guarded_void([&] {
+        cudaStream_t s = need_gpu();
+        const size_t Q = n_queries, nB = db->n_rows;
+        check_query_csr(q_hashes, q_offsets, Q);
+        if (Q == 0 || nB == 0) return;
+        const MvmPlan plan = many_vs_many_plan(q_offsets, Q, *db, s);
+        for (size_t c = 0; c + 1 < plan.cuts.size(); ++c) {
+            const size_t a = plan.cuts[c], b = plan.cuts[c + 1];
+            const uint64_t nk = q_offsets[b] - q_offsets[a];
+            DevBuf<uint64_t> d_q(nk, s);
+            d_q.upload(q_hashes + q_offsets[a], nk);
+            DevBuf<uint32_t> d_cnt((b - a) * nB, s);
+            d_cnt.zero();
+            many_vs_many_group(plan, d_q.p, q_offsets, a, b, *db, d_cnt.p, s);
+            d_cnt.download(counts_out + a * nB, (b - a) * nB);
+            sync(s);
+        }
+    });
+}
+
+void smb_many_vs_many_dev(const uint64_t* d_q_hashes, const uint64_t* q_offsets, uintptr_t n_queries,
+                          const SmbSketchSet* db, uint32_t* d_counts_out) {
+    guarded_void([&] {
+        cudaStream_t s = need_gpu();
+        const size_t Q = n_queries, nB = db->n_rows;
+        check_query_csr(nullptr, q_offsets, Q);
+        if (Q == 0 || q_offsets[Q] == 0) {
+            if (Q && nB) CK(cudaMemsetAsync(d_counts_out, 0, Q * nB * sizeof(uint32_t), s));
+            return;
+        }
+        {   // every query sorted and unique: one pass over the keys on the device
+            DevBuf<uint64_t> d_off(Q + 1, s);
+            DevBuf<unsigned long long> d_stat(2, s);
+            d_off.upload(q_offsets, Q + 1);
+            d_stat.zero();
+            smb::launch_query_stats(d_q_hashes, d_off.p, (int)Q, nullptr, d_stat.p, s);
+            CK(cudaGetLastError());
+            unsigned long long stat[2] = {0, 0};
+            d_stat.download(stat, 2);
+            sync(s);
+            if (stat[1]) fail(SOURMASH_ERROR_CODE_MSG, "every query must be sorted and unique");
+        }
+        if (nB == 0) return;
+        CK(cudaMemsetAsync(d_counts_out, 0, Q * nB * sizeof(uint32_t), s));
+        const MvmPlan plan = many_vs_many_plan(q_offsets, Q, *db, s);
+        for (size_t c = 0; c + 1 < plan.cuts.size(); ++c) {
+            const size_t a = plan.cuts[c], b = plan.cuts[c + 1];
+            many_vs_many_group(plan, d_q_hashes + q_offsets[a], q_offsets, a, b, *db, d_counts_out + a * nB, s);
+        }
     });
 }
 

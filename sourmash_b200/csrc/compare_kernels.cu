@@ -306,12 +306,60 @@ cudaError_t range_major_build(const u64* h, const u64* off, int n, u64 T, u64 ma
 }
 void range_major_destroy(RangeMajor* rm) { delete rm; }
 
-void launch_one_vs_many_range_major(const RangeMajor* rm, const u64* q, u64 nq, u32* out, cudaStream_t s) {
+// the pass over one key stream: one query (qid null) or the merged keys of a group (range_kernels.cuh)
+static void launch_range_major_pass(const RangeMajor* rm, const u64* q, const u32* qid, u64 nq, u32* out, cudaStream_t s) {
     if (nq == 0 || rm->n == 0) return;
-    RangeMajorArgs a{q, nq, (const u64*)rm->m_rm, (const u32*)rm->m_slice, (const u32*)rm->m_coarse, rm->nc, rm->n, rm->P, rm->width, (u32)RM_BITMAP_LOG2, rm->bm_shift, out};
+    RangeMajorArgs a{q, nq, (const u64*)rm->m_rm, (const u32*)rm->m_slice, (const u32*)rm->m_coarse, rm->nc, rm->n, rm->P, rm->width, (u32)RM_BITMAP_LOG2, rm->bm_shift, out, qid};
     const size_t smem = ((size_t)1 << (RM_BITMAP_LOG2 - 3)) + (size_t)(RM_THREADS / 32) * RM_QUEUE * sizeof(u32);
     cudaFuncSetAttribute(one_vs_many_range_major_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     one_vs_many_range_major_kernel<<<rm->P, RM_THREADS, smem, s>>>(a); count_launches(1);
+}
+void launch_one_vs_many_range_major(const RangeMajor* rm, const u64* q, u64 nq, u32* out, cudaStream_t s) {
+    launch_range_major_pass(rm, q, nullptr, nq, out, s);
+}
+
+// Query keys per range of one many-query group.  The bitmap alone would take 32 768 (two probes set at most 12 % of its
+// 2^19 bits), but the settled matches grow with the group: against configs[4] (every query with its own planted rows)
+// groups of 8 queries (1 060 keys per range) beat one pass per query on an H100, groups of 32 (4 240) and 128 (17 000)
+// were slower -- each match costs a binary search in the range's keys and a row attribution, done by one warp
+static constexpr u64 RM_GROUP_KEYS_PER_RANGE = 1024;
+u64 range_major_group_keys(const RangeMajor* rm) { return RM_GROUP_KEYS_PER_RANGE * (u64)rm->P; }
+
+void launch_query_stats(const u64* q, const u64* d_qoff, int G, u32* ids, unsigned long long* d_stat, cudaStream_t s) {
+    if (G <= 0) return;
+    rm_query_ids_kernel<<<std::min(G, SMB_SMS * 8), 256, 0, s>>>(q, d_qoff, G, ids, d_stat); count_launches(1);
+}
+
+cudaError_t many_vs_many_range_major(const RangeMajor* rm, const u64* q, const u64* d_qoff, int G, u64 n_keys,
+                                     u32* out, bool* unsorted, cudaStream_t s) {
+    *unsorted = false;
+    if (n_keys == 0 || rm->n == 0) return cudaSuccess;
+    JoinScratch scratch(s);
+    u64* keys = nullptr;
+    u32 *ids_in = nullptr, *ids = nullptr;
+    unsigned long long* d_stat = nullptr;
+    cudaError_t e;
+    if ((e = scratch.alloc((void**)&keys, n_keys * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&ids_in, n_keys * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&ids, n_keys * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&d_stat, 2 * sizeof(unsigned long long))) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(d_stat, 0, 2 * sizeof(unsigned long long), s)) != cudaSuccess) return e;
+    launch_query_stats(q, d_qoff, G, ids_in, d_stat, s);
+    unsigned long long stat[2] = {0, 0};
+    if ((e = cudaMemcpyAsync(stat, d_stat, sizeof(stat), cudaMemcpyDeviceToHost, s)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
+    if (stat[1]) { *unsorted = true; return cudaSuccess; }
+    int end_bit = 1;
+    while (end_bit < 64 && (stat[0] >> end_bit)) ++end_bit;
+    // stable: inside a run of equal keys the ids keep the query order
+    size_t sort_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, q, keys, ids_in, ids, (long long)n_keys, 0, end_bit, s);
+    void* d_sort = nullptr;
+    if ((e = scratch.alloc(&d_sort, sort_bytes)) != cudaSuccess) return e;
+    cub::DeviceRadixSort::SortPairs(d_sort, sort_bytes, q, keys, ids_in, ids, (long long)n_keys, 0, end_bit, s);
+    count_launches(1);
+    launch_range_major_pass(rm, keys, ids, n_keys, out, s);
+    return cudaGetLastError();
 }
 bool range_search_enabled() {
     const char* layout = getenv("SMB_SEARCH_LAYOUT");

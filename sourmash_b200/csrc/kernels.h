@@ -59,6 +59,16 @@ cudaError_t range_major_build(const uint64_t* h, const uint64_t* off, int n, uin
                               RangeMajor** out, cudaStream_t s);
 void range_major_destroy(RangeMajor* rm);
 void launch_one_vs_many_range_major(const RangeMajor* rm, const uint64_t* q, uint64_t nq, uint32_t* out, cudaStream_t s);
+// The same pass for a group of G queries, the database read once: q holds their keys back to back (d_qoff: G + 1
+// offsets from 0, on the device), out the G x n counters (query-major, zeroed by the caller).  The keys are merged by
+// a radix sort into one stream with the query ids alongside.  *unsorted is set, and nothing counted, when a query is
+// not sorted and unique.  range_major_group_keys bounds n_keys (the per-range bitmaps stay sparse).
+uint64_t range_major_group_keys(const RangeMajor* rm);
+cudaError_t many_vs_many_range_major(const RangeMajor* rm, const uint64_t* q, const uint64_t* d_qoff, int G, uint64_t n_keys,
+                                     uint32_t* out, bool* unsorted, cudaStream_t s);
+// stat[0] = max key, stat[1] > 0 iff a query of the CSR is not sorted and unique (ids: null, or the query of every key)
+void launch_query_stats(const uint64_t* q, const uint64_t* d_qoff, int G, uint32_t* ids, unsigned long long* d_stat,
+                        cudaStream_t s);
 
 // All-vs-all counts by inverted join (compare_kernels.cu): sort the (hash, row) pairs of the set,
 // one increment per pair of rows sharing a hash.  join_estimate sorts the lowest 1/JOIN_SAMPLE of

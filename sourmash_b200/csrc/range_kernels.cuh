@@ -14,6 +14,12 @@
 // per thread -- and probes the bitmap.  The rare hits (true matches + false positives) go to a per-warp queue and
 // are settled in bulk: exact binary search in the query's slice, then the row is found from `slice` and its counter
 // incremented.  Algorithmic bytes: 8 (|Q| + sum |S_j|), each read once.
+//
+// The same pass counts a GROUP of G queries at once (many_vs_many): their keys, concatenated and sorted by a stable
+// pair sort with the query id as the value, form one key stream with a parallel array of ids (ascending inside a run
+// of equal keys).  The bitmap is built from the stream's slice as before -- a key held by several queries sets the
+// same two bits again -- and a settled match adds 1 to counter (query, row) of every query in the key's run: the
+// database is read once for the whole group instead of once per query.
 #pragma once
 #include "common.cuh"
 #include "range_search.cuh"
@@ -90,7 +96,7 @@ __global__ void __launch_bounds__(256) rm_coarse_kernel(const u32* __restrict__ 
 }
 
 struct RangeMajorArgs {
-    const u64* q; u64 nq;                 // the query, sorted
+    const u64* q; u64 nq;                 // the query, sorted (a group of queries: their merged key stream, see qid)
     const u64* rm;                        // range-major database
     const u32* slice;                     // [P * n + 1]
     const u32* coarse; int nc;            // [P * nc]
@@ -98,7 +104,8 @@ struct RangeMajorArgs {
     u64 width;
     u32 bm_log2;                          // bits of the bitmap = 2^bm_log2 (RM_BITMAP_LOG2; tests use tiny bitmaps: false positives)
     u32 bm_shift;                         // (x - lo) >> bm_shift < 2^bm_log2
-    u32* out;                             // zeroed by the caller
+    u32* out;                             // zeroed by the caller: [n] counters, or [G x n] (query-major) with qid
+    const u32* qid;                       // null: one query; else the query of every key of q (a G-query group)
 };
 
 __device__ __forceinline__ u32 rm_bit1(u64 d, u32 bm_shift) { return (u32)(d >> bm_shift); }
@@ -119,7 +126,26 @@ __device__ __forceinline__ void rm_drain(const RangeMajorArgs& a, const u32* __r
         l <<= RM_COARSE_LOG2;
         r = l + (1 << RM_COARSE_LOG2) < a.n ? l + (1 << RM_COARSE_LOG2) : a.n;
         while (r - l > 1) { const int mid = (l + r) >> 1; if (slice_p[mid] <= pos) l = mid; else r = mid; }
-        atomicAdd(a.out + l, 1u);
+        // every query that holds x: the run of equal keys from lo (one query: the run is this key, the counter out[l])
+        u64 j = lo;
+        do atomicAdd(a.out + (a.qid ? (u64)a.qid[j] * (u64)a.n : 0ull) + l, 1u);
+        while (a.qid && ++j < qhi && a.q[j] == x);
+    }
+}
+
+// ids[k] = g for the keys k of query g of a group (qoff: its G + 1 offsets into the concatenated keys, from 0);
+// stat[0] = the largest key (the sort's significant bits), stat[1] > 0 iff a query is not sorted and unique
+__global__ void __launch_bounds__(256) rm_query_ids_kernel(const u64* __restrict__ q, const u64* __restrict__ qoff, int G,
+                                                          u32* __restrict__ ids, unsigned long long* __restrict__ stat) {
+    for (int g = blockIdx.x; g < G; g += gridDim.x) {
+        const u64 b = qoff[g], e = qoff[g + 1];
+        u32 bad = 0;
+        for (u64 k = b + threadIdx.x; k < e; k += blockDim.x) {
+            if (ids) ids[k] = (u32)g;
+            bad |= k > b && q[k] <= q[k - 1];
+        }
+        if (bad) atomicAdd(stat + 1, 1ull);
+        if (threadIdx.x == 0 && e > b) atomicMax(stat, (unsigned long long)q[e - 1]);
     }
 }
 

@@ -128,6 +128,11 @@ class LinearIndex:
     def find(self, search_fn, query, **kwargs):
         """Yield IndexSearchResult for subjects passing search_fn, in index order
         (Index.find, index/__init__.py:115-170)."""
+        yield from self._find(search_fn, query)
+
+    def _find(self, search_fn, query, counted=None, cache=None):
+        """find(); ``counted`` maps a resident group's key to (query size, shared counts) already computed for this
+        query by ``_many_counts`` (``cache``: its downsampled groups), the other groups are counted here."""
         search_fn.check_is_compatible(query)
         query_mh = query.minhash
         assert not query_mh.track_abundance
@@ -141,13 +146,16 @@ class LinearIndex:
                 if kind != "scaled":
                     raise ValueError("cannot compare scaled query against num sketches")
                 s = max(query_mh.scaled, val)
-                q = query_mh.downsample(scaled=s) if s > query_mh.scaled else query_mh
-                sub = sset.downsample(B.max_hash_for_scaled(s)) if s > val else sset
-                qarr = q._mins_array()
-                shared = B.one_vs_many(qarr, sub)
+                sub = self._downsampled(kind, val, sset, s, cache)
+                if counted is not None and (kind, val) in counted:
+                    n_query, shared = counted[(kind, val)]
+                else:
+                    q = query_mh.downsample(scaled=s) if s > query_mh.scaled else query_mh
+                    qarr = q._mins_array()
+                    n_query, shared = len(qarr), B.one_vs_many(qarr, sub)
                 sizes = sub.sizes()
-                total = len(qarr) + sizes - shared
-                qsize = np.full(len(indices), len(qarr))
+                total = n_query + sizes - shared
+                qsize = np.full(len(indices), n_query)
             else:
                 if kind != "num":
                     raise ValueError("cannot compare num query against scaled sketches")
@@ -170,6 +178,73 @@ class LinearIndex:
                 subj = self._subject(idx)
                 if search_fn.collect(score, subj):
                     yield IndexSearchResult(score, subj, self.location)
+
+    def _downsampled(self, kind, val, sset, s, cache=None):
+        "the resident group (kind, val) at scaled s >= val (cache: {(kind, val, s): SketchSet} shared across queries)"
+        if s <= val:
+            return sset
+        if cache is None:
+            return sset.downsample(B.max_hash_for_scaled(s))
+        key = (kind, val, s)
+        if key not in cache:
+            cache[key] = sset.downsample(B.max_hash_for_scaled(s))
+        return cache[key]
+
+    def _many_counts(self, queries):
+        """({query position: {group key: (query size, shared counts)}}, downsampled groups) for the queries the batched pass takes: flat
+        scaled queries compatible with every subject, against the scaled groups.  Each (group, effective scaled
+        s = max(query scaled, group scaled)) is one downsampled copy and one many_vs_many call.  Every other query
+        and group is counted by _find itself, query by query, with its errors."""
+        mhs = [q.minhash for q in queries]
+        ok = [i for i, mh in enumerate(mhs) if mh.scaled and not mh.track_abundance
+              and self._first_incompatible(mh) is None]
+        out = {i: {} for i in ok}
+        cache = {}
+        for (kind, val), (_indices, sset) in self._groups().items():
+            if kind != "scaled" or not ok:
+                continue
+            by_s = {}
+            for i in ok:
+                by_s.setdefault(max(mhs[i].scaled, val), []).append(i)
+            for s, members in by_s.items():
+                sub = self._downsampled(kind, val, sset, s, cache)
+                qarrs = [(mhs[i].downsample(scaled=s) if s > mhs[i].scaled else mhs[i])._mins_array() for i in members]
+                counts = B.many_vs_many(qarrs, sub)
+                for i, qarr, row in zip(members, qarrs, counts):
+                    out[i][(kind, val)] = (len(qarr), row)
+        return out, cache
+
+    def search_many(self, queries, *, threshold=None, do_containment=False, do_max_containment=False,
+                    best_only=False, **kwargs):
+        """search() of every query: element i equals ``self.search(queries[i], ...)``, the first query whose
+        search would raise raises the same here.  Queries that share a resident group and an effective scaled are
+        counted together, one pass over the group for many queries."""
+        if not queries:
+            return []
+        if threshold is None:
+            raise TypeError("'search' requires 'threshold'")
+        counted, cache = self._many_counts(queries)
+        out = []
+        for i, query in enumerate(queries):
+            search_obj = make_jaccard_search_query(do_containment=do_containment,
+                                                   do_max_containment=do_max_containment,
+                                                   best_only=best_only, threshold=float(threshold))
+            matches = list(self._find(search_obj, query, counted.get(i), cache))
+            matches.sort(key=lambda x: -x.score)
+            out.append(matches)
+        return out
+
+    def prefetch_many(self, queries, threshold_bp, **kwargs):
+        """prefetch() of every query: element i equals ``list(self.prefetch(queries[i], threshold_bp))``, the first
+        query whose prefetch would raise raises the same here.  Counted as in search_many."""
+        if not queries:
+            return []
+        if not self:
+            raise ValueError("no signatures to search")
+        counted, cache = self._many_counts(queries)
+        return [list(self._find(make_containment_query(query.minhash, threshold_bp, best_only=False), query,
+                                counted.get(i), cache))
+                for i, query in enumerate(queries)]
 
     def search_abund(self, query, *, threshold=None, **kwargs):
         """Matches by angular similarity of abundance sketches, best first (Index.search_abund, index/__init__.py:172-200):
