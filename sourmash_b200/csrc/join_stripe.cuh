@@ -240,8 +240,8 @@ __device__ __forceinline__ void stripe_inc_if(StripeRowRef row, u32 col, bool on
 // One CTA = rows [r0, r1) of the result.  Work items are (row, chunk of 32 consecutive elements), handed to the
 // warps chunk index first, so that all rows of the CTA -- and, as CTAs start together, all CTAs of a wave --
 // move through the hash-ordered stream together.  For every element with a successor in its group the warp
-// reads the 32 tags behind it (four elements' reads in flight) and the lanes in front of the next group head
-// increment their counters.  UPPER: only later members (= higher rows) are counted, i.e. the cells (i, j > i);
+// reads the 32 tags behind it (two elements' reads in flight), and 32 more while no group head has turned up; the
+// lanes in front of the next group head increment their counters.  UPPER: only later members (= higher rows) are counted, i.e. the cells (i, j > i);
 // stripe_mirror_kernel fills the rest.  Otherwise the members in front are counted too (full rows, used when a
 // block of rows is computed on its own).
 template <typename TagT, bool UPPER, int CTAS>
@@ -267,9 +267,6 @@ __global__ void __launch_bounds__(1024, CTAS) join_stripe_kernel(StripeArgs a) {
     const u32 n_items = s_ctl[1] * (u32)rows;
     const u32 le_mask = (2u << lane) - 1u;                // lanes <= lane
     const u32 lt_mask = (1u << lane) - 1u;                // lanes <  lane
-    // tags[q + 1 + lane]: the stream is padded with head flags behind its end (stripe_tag_kernel), and T < 2^32 - 128,
-    // so forward reads need no bounds checks and 32-bit positions do not wrap
-    const TagT* __restrict__ fwd = tags + 1 + lane;
 
     for (;;) {
         u32 k = 0;
@@ -285,11 +282,14 @@ __global__ void __launch_bounds__(1024, CTAS) join_stripe_kernel(StripeArgs a) {
         const u32 my_q = have ? ld_stream_u32(a.pos + e) : 0u;
         u32* row_ptr = stripe + (size_t)r * n;
 
-        // ---- members behind the element (higher rows): 64 tags per element are requested at once (groups of
-        // the benchmark have ~35 members behind an element on average), two elements per round.  A lane counts
-        // its tag when no group head lies at or in front of it (m & le_mask == 0); a tag is the stripe column of its row
-        // (stripe_col), and that of a tag that is not counted is still a valid column (the padding tags are HEAD | 0), so
-        // addresses need no guard.
+        // ---- members behind the element (higher rows): the 32 tags behind it, two elements' reads in flight per
+        // round, then 32 more at a time only while no group head has turned up.  The kernel is bound by the sectors it
+        // reads from L2 / HBM, not by the latency of a read: reading 64 tags up front (the benchmark's elements
+        // have ~29 members behind them on average) fetched tags past the group's end that nobody counts.  A lane
+        // counts its tag when no group head lies at or in front of it (m & le_mask == 0); a tag is the stripe column of
+        // its row (stripe_col), and that of a tag that is not counted is still a valid column (the padding tags are
+        // HEAD | 0), so addresses need no guard.  Every read lies inside the STRIPE_TAG_PAD head flags behind the stream:
+        // a read of 32 tags is only issued when the previous one ended inside the group, whose end is at most T.
         const StripeRowRef row_ref = stripe_row_ref(row_ptr);
         const u32 lane1 = lane + 1u;
         u32 nxt = HEAD;
@@ -304,33 +304,23 @@ __global__ void __launch_bounds__(1024, CTAS) join_stripe_kernel(StripeArgs a) {
             // 32-bit position + lane + 1 (no wrap: T < 2^32 - 128), widened once per element
             const TagT* __restrict__ p0 = tags + (__shfl_sync(0xffffffffu, my_q, j0) + lane1);
             const TagT* __restrict__ p1 = tags + (__shfl_sync(0xffffffffu, my_q, j1) + lane1);
-            const u32 t00 = (u32)p0[0], t01 = (u32)p0[32];
-            u32 t10 = HEAD, t11 = HEAD;
-            if (two) { t10 = (u32)p1[0]; t11 = (u32)p1[32]; }
-            {
-                u32 m = __ballot_sync(0xffffffffu, t00 >= HEAD);
-                stripe_inc_if(row_ref, t00 & (HEAD - 1u), (m & le_mask) == 0);
-                if (m == 0) {
-                    m = __ballot_sync(0xffffffffu, t01 >= HEAD);
-                    stripe_inc_if(row_ref, t01 & (HEAD - 1u), (m & le_mask) == 0);
-                    for (u32 it = 2; m == 0; ++it) {       // more than 64 members behind
-                        const u32 tt = (u32)p0[32 * it];
-                        m = __ballot_sync(0xffffffffu, tt >= HEAD);
-                        stripe_inc_if(row_ref, tt & (HEAD - 1u), (m & le_mask) == 0);
-                    }
-                }
+            const u32 t0 = (u32)p0[0];
+            u32 t1 = HEAD;
+            if (two) t1 = (u32)p1[0];
+            u32 m = __ballot_sync(0xffffffffu, t0 >= HEAD);
+            stripe_inc_if(row_ref, t0 & (HEAD - 1u), (m & le_mask) == 0);
+            for (u32 it = 1; m == 0; ++it) {               // more than 32 members behind
+                const u32 tt = (u32)p0[32 * it];
+                m = __ballot_sync(0xffffffffu, tt >= HEAD);
+                stripe_inc_if(row_ref, tt & (HEAD - 1u), (m & le_mask) == 0);
             }
             if (two) {
-                u32 m = __ballot_sync(0xffffffffu, t10 >= HEAD);
-                stripe_inc_if(row_ref, t10 & (HEAD - 1u), (m & le_mask) == 0);
-                if (m == 0) {
-                    m = __ballot_sync(0xffffffffu, t11 >= HEAD);
-                    stripe_inc_if(row_ref, t11 & (HEAD - 1u), (m & le_mask) == 0);
-                    for (u32 it = 2; m == 0; ++it) {
-                        const u32 tt = (u32)p1[32 * it];
-                        m = __ballot_sync(0xffffffffu, tt >= HEAD);
-                        stripe_inc_if(row_ref, tt & (HEAD - 1u), (m & le_mask) == 0);
-                    }
+                m = __ballot_sync(0xffffffffu, t1 >= HEAD);
+                stripe_inc_if(row_ref, t1 & (HEAD - 1u), (m & le_mask) == 0);
+                for (u32 it = 1; m == 0; ++it) {
+                    const u32 tt = (u32)p1[32 * it];
+                    m = __ballot_sync(0xffffffffu, tt >= HEAD);
+                    stripe_inc_if(row_ref, tt & (HEAD - 1u), (m & le_mask) == 0);
                 }
             }
         }
