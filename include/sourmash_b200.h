@@ -430,6 +430,27 @@ SmbSketchSet *smb_sketch_records(const SmbRecords *r, const uint32_t *rec_to_ske
                                  uint32_t num, uint64_t seed, bool track_abundance,
                                  uint64_t *n_kmers_out);
 
+/* `sig kmers` over a batch of records: every window of every record is hashed as add_sequence(seq, force=True) /
+ * add_protein (input_is_protein) would, and each window whose hash is in `query` (sorted-unique, the merged sketch's
+ * hashes; for num sketches its bottom num) becomes one match (key, hash), key = record << 32 | ordinal, ordinal = the
+ * window's index in seq_to_hashes order.  Matches come sorted by key.  Per record: matched = seq_mh.intersection(query)
+ * is not empty (num sketches: kmerminhash_intersection), has_invalid = a DNA window holds a non-ACGT base.  found = the
+ * query hashes of found_mh += seq_mh.intersection(query_mh) over the matched records, sorted.  ksize as stored (3 x
+ * residues for protein-family sketches); max_hash for scaled sketches, num for num sketches.  skip_invalid: records with
+ * has_invalid add nothing to found (`--check-sequence --force` skips them). */
+typedef struct SmbKmerMatches SmbKmerMatches;
+SmbKmerMatches *smb_kmer_match_records(const SmbRecords *r, const uint64_t *query, uintptr_t n_query, uint32_t ksize,
+                                       HashFunctions hash_function, uint64_t seed, uint64_t max_hash, uint32_t num,
+                                       bool input_is_protein, bool skip_invalid);
+uintptr_t smb_kmer_matches_len(const SmbKmerMatches *m);
+const uint64_t *smb_kmer_matches_keys(const SmbKmerMatches *m);          /* len */
+const uint64_t *smb_kmer_matches_hashes(const SmbKmerMatches *m);        /* len */
+const uint8_t *smb_kmer_matches_matched(const SmbKmerMatches *m);        /* one per record */
+const uint8_t *smb_kmer_matches_has_invalid(const SmbKmerMatches *m);    /* one per record */
+uintptr_t smb_kmer_matches_n_found(const SmbKmerMatches *m);
+const uint64_t *smb_kmer_matches_found(const SmbKmerMatches *m);
+void smb_kmer_matches_free(SmbKmerMatches *m);
+
 /* Signature objects straight from a sketch set (the tail of _compute_individual,
  * command_sketch.py:770-789): signature g owns rows [g * n_ksizes, (g + 1) * n_ksizes); ksizes
  * are the ABI values.  Array freed with signatures_array_free, objects with signature_free. */

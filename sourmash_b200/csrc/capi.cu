@@ -2952,6 +2952,184 @@ SmbSketchSet* smb_sketch_records(const SmbRecords* r, const uint32_t* rec_to_ske
     });
 }
 
+// `sig kmers` over a batch of records (sig/__main__.py:1206-1256): every window of every record hashed and probed against
+// the merged query on the device (kmer_match_kernels.cuh), the matches sorted into file order, the per-record flags and
+// the found hashes of the query.  query: sorted-unique hashes of the merged sketch (for num sketches its bottom num).
+struct SmbKmerMatches {
+    std::vector<uint64_t> keys, hashes, found;
+    std::vector<uint8_t> matched, has_invalid;
+};
+
+SmbKmerMatches* smb_kmer_match_records(const SmbRecords* r, const uint64_t* query, uintptr_t n_query, uint32_t ksize,
+                                       HashFunctions hash_function, uint64_t seed, uint64_t max_hash, uint32_t num,
+                                       bool input_is_protein, bool skip_invalid) {
+    return guarded<SmbKmerMatches*>([&]() -> SmbKmerMatches* {
+        const smb::RecordBatch& b = r->b;
+        const size_t n = b.file.size();
+        cudaStream_t s = need_gpu();
+        for (uintptr_t i = 1; i < n_query; ++i)
+            if (query[i] <= query[i - 1]) fail(SOURMASH_ERROR_CODE_MSG, "query hashes must be sorted and unique");
+        if (n >= (1ull << 32)) fail(SOURMASH_ERROR_CODE_MSG, "more than 2^32 - 1 records in one batch");
+        const bool dna = hash_function == HASH_FUNCTIONS_MURMUR64_DNA;
+        if (dna && input_is_protein)
+            fail(SOURMASH_ERROR_CODE_INVALID_HASH_FUNCTION, "Invalid hash function: \"DNA\"");   // signature.rs:376-380
+        const uint32_t kaa = ksize / 3;
+        const bool translate = !dna && !input_is_protein;
+        if (!dna && kaa > smb::aa_max_k(translate))
+            fail(SOURMASH_ERROR_CODE_INTERNAL, "protein-family ksize too large for the shared-memory tile");
+        auto res = std::make_unique<SmbKmerMatches>();
+        res->matched.assign(n, 0);
+        res->has_invalid.assign(n, 0);
+        const bool stores = num > 0 || max_hash > 0;                 // minhash.rs:324-327
+        if (n == 0 || n_query == 0 || !stores) return res.release();
+
+        // chunks of W windows (window starts) per record; the ordinal of a window must fit 32 bits
+        smb::KmerMatchArgs a{};
+        a.mode = dna ? (smb::k_has_rolled_kernel(ksize) ? 0 : 1) : (translate ? 3 : 2);
+        a.K = dna ? ksize : kaa;
+        a.W = a.mode == 0 ? 32 : 8;
+        std::vector<uint64_t> chunk(n + 1, 0);
+        uint64_t n_windows = 0;
+        for (size_t i = 0; i < n; ++i) {
+            const uint64_t L = b.len[i];
+            uint64_t starts = 0, wins = 0, span_bytes = 0;
+            if (dna) { starts = ksize && L >= ksize ? L - ksize + 1 : 0; wins = starts; }
+            else { const uint64_t span = translate ? 3ull * kaa : kaa; starts = kaa && L >= span ? L - span + 1 : 0;
+                   wins = translate ? 2 * starts : starts; }
+            if (wins >= (1ull << 32)) fail(SOURMASH_ERROR_CODE_MSG, "record " + std::to_string(i) + " has 2^32 or more k-mers");
+            // rolled kernel: chunks tile the record's aligned coordinates (hash_thread_windows)
+            span_bytes = a.mode == 0 ? (starts ? (b.start[i] & 15) + L : 0) : starts;
+            chunk[i + 1] = chunk[i] + (span_bytes + a.W - 1) / a.W;
+            n_windows += wins;
+        }
+        DevBuf<uint8_t> d_bases(b.extent + 32, s);
+        d_bases.upload(b.seqs, b.extent);
+        DevBuf<uint64_t> d_off(n, s), d_len(n, s), d_chunk(n + 1, s), d_q(n_query, s);
+        d_off.upload(b.start.data(), n);
+        d_len.upload(b.len.data(), n);
+        d_chunk.upload(chunk.data(), n + 1);
+        d_q.upload(query, n_query);
+        DevBuf<uint8_t> d_hit(n, s), d_invalid(n, s), d_tabs;
+        d_hit.zero(); d_invalid.zero();
+        if (!dna) {
+            const smb::AaTables T = smb::build_aa_tables((int)hash_function);
+            d_tabs.alloc(sizeof T, s);
+            d_tabs.upload((const uint8_t*)&T, sizeof T);
+            sync(s);                                                 // T is a stack temporary
+        }
+        a.bases = d_bases.p; a.rec_off = d_off.p; a.rec_len = d_len.p; a.chunk_start = d_chunk.p;
+        a.n_chunks = chunk[n]; a.n_rec = (int)n;
+        a.seed = seed; a.max_hash = num > 0 ? UINT64_MAX : max_hash;
+        a.tabs = (const smb::AaTables*)d_tabs.p;
+        a.rec_hit = d_hit.p; a.rec_invalid = dna ? d_invalid.p : nullptr;
+        // Q: UINT64_MAX answered by a flag, the rest by the split table (small Q) or the global directory
+        a.q_has_max = query[n_query - 1] == UINT64_MAX;
+        a.q = d_q.p; a.nq = n_query - (a.q_has_max ? 1 : 0);
+        a.q_top = a.nq ? query[a.nq - 1] : 0;
+        DevBuf<uint32_t> d_dir, d_bm;
+        a.split = smb::kmer_match_split_fits(a.nq);
+        if (a.split) {
+            const uint64_t entries = std::max<uint64_t>(a.nq, 256);          // about one key per bucket
+            uint32_t sh = 0;
+            while (sh < 63 && (a.q_top >> sh) >= entries) ++sh;
+            a.shift = sh; a.nb = (a.q_top >> sh) + 1;
+        } else {
+            int nb_log2 = 12;                                              // as one_vs_many_dev
+            while (nb_log2 < 26 && (1ull << nb_log2) < 2 * a.nq) ++nb_log2;
+            uint32_t sh = 0;
+            while (sh < 63 && (a.q_top >> sh) >= (1ull << nb_log2)) ++sh;
+            a.shift = sh; a.nb = (a.q_top >> sh) + 1;
+            d_dir.alloc(a.nb + 2, s);
+            smb::launch_build_global_dir(d_q.p, a.nq, (int)sh, a.nb, d_dir.p, s);
+            a.fine_log2 = 3;
+            d_bm.alloc(((size_t)a.nb << a.fine_log2) / 32 + 2, s);
+            d_bm.zero();
+            smb::launch_build_query_bitmap(d_q.p, a.nq, (int)sh, a.fine_log2, d_bm.p, s);
+            a.gdir = d_dir.p; a.bitmap = d_bm.p;
+        }
+        // match buffer: room for about four times the expected probes' worth of hits; an overflow reruns at the exact size
+        const long double probes = num > 0 ? (long double)n_windows
+                                           : (long double)n_windows * (((long double)max_hash + 1.0L) / 18446744073709551616.0L);
+        uint64_t cap = (uint64_t)std::min<long double>((long double)n_windows, probes + 4.0L * n_query + 4096.0L);
+        DevBuf<unsigned long long> d_count(1, s);
+        DevBuf<uint64_t> d_keys, d_hashes;
+        unsigned long long count = 0;
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            d_keys.alloc(cap, s); d_hashes.alloc(cap, s);
+            d_count.zero();
+            a.keys = d_keys.p; a.hashes = d_hashes.p; a.cap = cap; a.count = d_count.p;
+            if (t_profiling) t_timer_hash.begin(s);
+            smb::launch_kmer_match(a, s);
+            if (t_profiling) t_timer_hash.end(s);
+            CK(cudaGetLastError());
+            d_count.download(&count, 1);
+            sync(s);
+            if (count <= cap) break;
+            cap = count;                                              // rerun with the exact count
+        }
+        if (count > cap) fail(SOURMASH_ERROR_CODE_INTERNAL, "k-mer match buffer overflowed twice");
+        // file order: one radix sort of (record << 32 | ordinal, hash)
+        const uint64_t m = count;
+        DevBuf<uint64_t> d_keys2(m, s), d_hashes2(m, s);
+        if (m) {
+            int end_bit = 33;
+            while (end_bit < 64 && (n >> (end_bit - 32)) != 0) ++end_bit;
+            CK(smb::sort_kmer_matches(d_keys.p, d_hashes.p, d_keys2.p, d_hashes2.p, m, end_bit, s));
+        }
+        // found hashes: for a scaled query every match; for a num query the common hashes of the passing records.
+        // skip_invalid: records with an invalid DNA window add nothing (`sig kmers --check-sequence --force` skips them)
+        const uint8_t* skip = skip_invalid && dna ? d_invalid.p : nullptr;
+        DevBuf<uint8_t> d_flag(n_query, s);
+        d_flag.zero();
+        if (num == 0) {
+            smb::launch_match_mark_found(d_keys2.p, d_hashes2.p, m, skip, d_q.p, n_query, d_flag.p, s);
+        } else {
+            d_hit.download(res->matched.data(), n);
+            sync(s);
+            std::vector<uint32_t> recs;
+            for (size_t i = 0; i < n; ++i) if (res->matched[i]) recs.push_back((uint32_t)i);
+            if (!recs.empty()) {
+                StreamList in;
+                in.d_bases = d_bases.p;
+                in.n_sketches = recs.size();
+                for (uint32_t i : recs) { in.off.push_back(b.start[i]); in.len.push_back(b.len[i]); }
+                SketchParams P;
+                P.ksizes = {ksize}; P.num = num; P.seed = seed;
+                P.hash_function = hash_function; P.input_is_protein = input_is_protein;
+                const bool prof = t_profiling;
+                t_profiling = false;                                 // the timer keeps the match pass
+                auto bottom = sketch_streams(in, P, s, nullptr);
+                t_profiling = prof;
+                DevBuf<uint32_t> d_recs(recs.size(), s);
+                d_recs.upload(recs.data(), recs.size());
+                smb::launch_match_num_common(bottom->d_hashes, bottom->d_off, d_recs.p, (int)recs.size(), d_q.p, n_query,
+                                             num, skip, d_hit.p, d_flag.p, s);
+                CK(cudaGetLastError());
+                sync(s);                                             // recs is a host temporary
+            }
+        }
+        CK(cudaGetLastError());
+        res->keys.resize(m); res->hashes.resize(m);
+        std::vector<uint8_t> flag(n_query);
+        d_keys2.download(res->keys.data(), m);
+        d_hashes2.download(res->hashes.data(), m);
+        d_hit.download(res->matched.data(), n);
+        if (dna) d_invalid.download(res->has_invalid.data(), n);
+        d_flag.download(flag.data(), n_query);
+        sync(s);
+        for (uintptr_t i = 0; i < n_query; ++i) if (flag[i]) res->found.push_back(query[i]);
+        return res.release();
+    });
+}
+uintptr_t smb_kmer_matches_len(const SmbKmerMatches* m) { return m->keys.size(); }
+const uint64_t* smb_kmer_matches_keys(const SmbKmerMatches* m) { return m->keys.data(); }
+const uint64_t* smb_kmer_matches_hashes(const SmbKmerMatches* m) { return m->hashes.data(); }
+const uint8_t* smb_kmer_matches_matched(const SmbKmerMatches* m) { return m->matched.data(); }
+const uint8_t* smb_kmer_matches_has_invalid(const SmbKmerMatches* m) { return m->has_invalid.data(); }
+uintptr_t smb_kmer_matches_n_found(const SmbKmerMatches* m) { return m->found.size(); }
+const uint64_t* smb_kmer_matches_found(const SmbKmerMatches* m) { return m->found.data(); }
+void smb_kmer_matches_free(SmbKmerMatches* m) { delete m; }
+
 // signatures straight from a sketch set (the tail of _compute_individual, command_sketch.py:770-789):
 // signature s gets rows [s * n_ksizes, (s + 1) * n_ksizes) of `set` as its sketches
 SourmashSignature** smb_signatures_from_sketchset(const SmbSketchSet* set, const uint32_t* ksizes,

@@ -271,6 +271,52 @@ void launch_angular_terms(const uint64_t* a, const uint64_t* aa, uint64_t na, co
 void launch_row_prefix_counts(const uint64_t* h, const uint64_t* off, int n_rows,
                               uint64_t max_hash, uint32_t* out_cnt, cudaStream_t s);
 
+// `sig kmers` (kmer_match_kernels.cuh): every window of every record hashed, the windows whose hash is in Q emitted as
+// (record << 32 | ordinal, hash); ordinal = the window's index in seq_to_hashes order.  The caller fills the arguments
+// (chunks of W windows per record, the probe layout, zeroed results); the launch picks the kernel from mode / K.
+struct KmerMatchArgs {
+    const uint8_t* bases;               // 16-byte aligned, readable up to the next 16-byte boundary past the end
+    const uint64_t* rec_off;            // [n_rec] byte offset of every record
+    const uint64_t* rec_len;            // [n_rec]
+    const uint64_t* chunk_start;        // [n_rec + 1] prefix of the chunks of every record
+    uint64_t n_chunks;
+    int n_rec, W;                       // W: windows (window starts) per chunk
+    int mode;                           // 0 rolled DNA (K = 21, 31, 51), 1 any other DNA k, 2 residues, 3 translated DNA
+    uint32_t K;                         // DNA: k; protein family: residues per window
+    uint64_t seed, max_hash;            // max_hash: UINT64_MAX for num sketches
+    // Q
+    const uint64_t* q;                  // sorted-unique, without a trailing UINT64_MAX
+    uint64_t nq, q_top;                 // q_top = q[nq - 1] (0 when nq == 0)
+    int q_has_max;                      // Q holds UINT64_MAX
+    int split;                          // 1: shared-memory split table of nq keys; 0: global directory
+    uint32_t shift;                     // bucket = key >> shift, buckets [0, nb)
+    uint64_t nb;
+    const uint32_t* gdir;               // global directory (nb + 1 entries) ...
+    const uint32_t* bitmap;             // ... and occupancy bitmap at 2^fine_log2 times its resolution
+    int fine_log2;
+    const AaTables* tabs;
+    // results
+    uint64_t* keys; uint64_t* hashes; uint64_t cap;
+    unsigned long long* count;          // matches found (may exceed cap)
+    uint8_t* rec_hit;                   // [n_rec] at least one match
+    uint8_t* rec_invalid;               // [n_rec] DNA: a window holds a non-ACGT byte (nullable)
+};
+bool kmer_match_split_fits(uint64_t nq);        // Q this large fits the shared-memory split table
+// (key, hash) pairs sorted by the key bits [0, end_bit), into the *_out arrays
+cudaError_t sort_kmer_matches(const uint64_t* keys, const uint64_t* hashes, uint64_t* keys_out, uint64_t* hashes_out,
+                              uint64_t m, int end_bit, cudaStream_t s);
+void launch_kmer_match(const KmerMatchArgs& a, cudaStream_t s);
+// found hashes of a scaled query: flag[i] = 1 when some match holds q[i]; matches of records with skip[r] != 0 (nullable)
+// do not count
+void launch_match_mark_found(const uint64_t* keys, const uint64_t* hashes, uint64_t n, const uint8_t* skip,
+                             const uint64_t* q, uint64_t nq, uint8_t* flag, cudaStream_t s);
+// num query: record recs[i] (bottom-num sketch = row i of bh / boff) passes when a hash common with Q is among the first
+// num of the union; rec_hit[recs[i]] is set to the result, flag[j] = 1 for the common q[j] of passing records that are
+// not skipped (skip[recs[i]] != 0, nullable)
+void launch_match_num_common(const uint64_t* bh, const uint64_t* boff, const uint32_t* recs, int n, const uint64_t* q,
+                             uint64_t nq, uint32_t num, const uint8_t* skip, uint8_t* rec_hit, uint8_t* flag,
+                             cudaStream_t s);
+
 // kernel-launch accounting (smb_kernel_launches)
 void count_launches(int n);
 

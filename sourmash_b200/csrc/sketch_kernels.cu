@@ -24,6 +24,7 @@
 #include "kmer_roll.cuh"
 #include "sketch_device.cuh"
 #include "aa_kmers.cuh"
+#include "kmer_match_kernels.cuh"
 
 namespace smb {
 
@@ -33,6 +34,46 @@ namespace smb {
 __device__ __forceinline__ u32 up_byte(u32 x) { return (x >= 'a' && x <= 'z') ? x - 32u : x; }
 __device__ __forceinline__ bool valid_base(u32 u) { return u == 'A' || u == 'C' || u == 'G' || u == 'T'; }
 __device__ __forceinline__ u32 comp_base(u32 u) { return u == 'A' ? 'T' : u == 'C' ? 'G' : u == 'G' ? 'C' : 'A'; }
+
+// one window of any k: validity of its k bytes and the murmur3 of the canonical k-mer (0 when invalid)
+__device__ __forceinline__ u64 dna_window_hash(const u8* __restrict__ base, u64 w, u32 K, u64 seed, bool& valid) {
+    valid = true;
+    for (u32 t = 0; t < K; ++t) valid = valid && valid_base(up_byte(base[w + t]));
+    if (!valid) return 0;
+    bool fwd = true;
+    for (u32 t = 0; t < K; ++t) {
+        u32 f = up_byte(base[w + t]), r = comp_base(up_byte(base[w + K - 1 - t]));
+        if (f != r) { fwd = f < r; break; }
+    }
+    auto at = [&](u32 t) -> u64 {
+        return fwd ? up_byte(base[w + t]) : comp_base(up_byte(base[w + K - 1 - t]));
+    };
+    u64 h1 = seed, h2 = seed;
+    const u32 nblk = K / 16;
+    for (u32 b = 0; b < nblk; ++b) {
+        u64 k1 = 0, k2 = 0;
+        for (int i = 7; i >= 0; --i) { k1 = (k1 << 8) | at(16 * b + i); k2 = (k2 << 8) | at(16 * b + 8 + i); }
+        k1 *= SMB_C1; k1 = smb_rotl64(k1, 31); k1 *= SMB_C2; h1 ^= k1;
+        h1 = smb_rotl64(h1, 27); h1 += h2; h1 = h1 * 5 + 0x52dce729ULL;
+        k2 *= SMB_C2; k2 = smb_rotl64(k2, 33); k2 *= SMB_C1; h2 ^= k2;
+        h2 = smb_rotl64(h2, 31); h2 += h1; h2 = h2 * 5 + 0x38495ab5ULL;
+    }
+    const u32 tail = K & 15u, tb = 16 * nblk;
+    if (tail > 8) {
+        u64 k2 = 0;
+        for (u32 i = tail; i > 8; --i) k2 = (k2 << 8) | at(tb + i - 1);
+        k2 *= SMB_C2; k2 = smb_rotl64(k2, 33); k2 *= SMB_C1; h2 ^= k2;
+    }
+    if (tail > 0) {
+        u64 k1 = 0;
+        for (u32 i = tail < 8 ? tail : 8; i > 0; --i) k1 = (k1 << 8) | at(tb + i - 1);
+        k1 *= SMB_C1; k1 = smb_rotl64(k1, 31); k1 *= SMB_C2; h1 ^= k1;
+    }
+    h1 ^= (u64)K; h2 ^= (u64)K;
+    h1 += h2; h2 += h1;
+    h1 = smb_fmix64(h1); h2 = smb_fmix64(h2);
+    return h1 + h2;
+}
 
 template <bool RAW>
 __global__ void __launch_bounds__(256) hash_kmers_generic_kernel(HashArgs a, u32 K) {
@@ -49,44 +90,8 @@ __global__ void __launch_bounds__(256) hash_kmers_generic_kernel(HashArgs a, u32
     if (w >= nwin) return;
     const int sk = a.stream_row ? (int)a.stream_row[stream] : stream;
     const int row = sk * a.row_stride + a.row_index;
-    bool valid = true;
-    for (u32 t = 0; t < K; ++t) valid = valid && valid_base(up_byte(base[w + t]));
-    u64 h = 0;
-    if (valid) {
-        bool fwd = true;
-        for (u32 t = 0; t < K; ++t) {
-            u32 f = up_byte(base[w + t]), r = comp_base(up_byte(base[w + K - 1 - t]));
-            if (f != r) { fwd = f < r; break; }
-        }
-        auto at = [&](u32 t) -> u64 {
-            return fwd ? up_byte(base[w + t]) : comp_base(up_byte(base[w + K - 1 - t]));
-        };
-        u64 h1 = a.seed, h2 = a.seed;
-        const u32 nblk = K / 16;
-        for (u32 b = 0; b < nblk; ++b) {
-            u64 k1 = 0, k2 = 0;
-            for (int i = 7; i >= 0; --i) { k1 = (k1 << 8) | at(16 * b + i); k2 = (k2 << 8) | at(16 * b + 8 + i); }
-            k1 *= SMB_C1; k1 = smb_rotl64(k1, 31); k1 *= SMB_C2; h1 ^= k1;
-            h1 = smb_rotl64(h1, 27); h1 += h2; h1 = h1 * 5 + 0x52dce729ULL;
-            k2 *= SMB_C2; k2 = smb_rotl64(k2, 33); k2 *= SMB_C1; h2 ^= k2;
-            h2 = smb_rotl64(h2, 31); h2 += h1; h2 = h2 * 5 + 0x38495ab5ULL;
-        }
-        const u32 tail = K & 15u, tb = 16 * nblk;
-        if (tail > 8) {
-            u64 k2 = 0;
-            for (u32 i = tail; i > 8; --i) k2 = (k2 << 8) | at(tb + i - 1);
-            k2 *= SMB_C2; k2 = smb_rotl64(k2, 33); k2 *= SMB_C1; h2 ^= k2;
-        }
-        if (tail > 0) {
-            u64 k1 = 0;
-            for (u32 i = tail < 8 ? tail : 8; i > 0; --i) k1 = (k1 << 8) | at(tb + i - 1);
-            k1 *= SMB_C1; k1 = smb_rotl64(k1, 31); k1 *= SMB_C2; h1 ^= k1;
-        }
-        h1 ^= (u64)K; h2 ^= (u64)K;
-        h1 += h2; h2 += h1;
-        h1 = smb_fmix64(h1); h2 = smb_fmix64(h2);
-        h = h1 + h2;
-    }
+    bool valid;
+    const u64 h = dna_window_hash(base, w, K, a.seed, valid);
     if (RAW) {
         a.raw_out[w] = valid ? h : 0ull;
     } else if (valid && h != 0ull && h <= a.max_hash) {
@@ -268,6 +273,66 @@ void launch_aa_window_hashes(const HashLaunch& L, const AaTables* d_tables, uint
     HashArgs a = make_hash_args(L, false, 0);
     a.stream_row = nullptr; a.row_stride = 1; a.row_index = 0; a.raw_out = raw_out;
     launch_hash_aa<true>(a, d_tables, kaa, translate, aa_frames(len, kaa), L.total_tiles_generic, s);
+}
+
+// ---------------------------------------------------------------------------------------
+// `sig kmers`: fused hash + probe over all records (kmer_match_kernels.cuh)
+// ---------------------------------------------------------------------------------------
+// The split table must leave room for two CTAs per SM next to the staging: keys (8 B each) up to 128 KB.
+bool kmer_match_split_fits(uint64_t nq) { return nq <= 16382; }
+
+template <int MODE, int K>
+static void launch_match_t(const KmerMatchArgs& a, cudaStream_t s) {
+    size_t smem = a.split ? match_split_smem(a.nq, a.nb) : 0;
+    if (MODE >= 2) smem = ((smem + 15) & ~(size_t)15) + sizeof(AaTables);
+    cudaFuncSetAttribute(kmer_match_kernel<MODE, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    const size_t per_cta = smem + (size_t)MATCH_STAGE * 16 + 1024;
+    u64 ctas_per_sm = (u64)(220 * 1024) / per_cta;
+    ctas_per_sm = ctas_per_sm < 1 ? 1 : ctas_per_sm > 4 ? 4 : ctas_per_sm;
+    u64 blocks = (a.n_chunks + MATCH_THREADS - 1) / MATCH_THREADS;
+    if (blocks > (u64)SMB_SMS * ctas_per_sm) blocks = (u64)SMB_SMS * ctas_per_sm;
+    kmer_match_kernel<MODE, K><<<(unsigned)blocks, MATCH_THREADS, smem, s>>>(a);
+    count_launches(1);
+}
+
+void launch_kmer_match(const KmerMatchArgs& a, cudaStream_t s) {
+    if (a.n_chunks == 0) return;
+    switch (a.mode) {
+        case 0:
+            if (a.K == 21) launch_match_t<0, 21>(a, s);
+            else if (a.K == 31) launch_match_t<0, 31>(a, s);
+            else launch_match_t<0, 51>(a, s);
+            break;
+        case 1: launch_match_t<1, 0>(a, s); break;
+        case 2: launch_match_t<2, 0>(a, s); break;
+        default: launch_match_t<3, 0>(a, s); break;
+    }
+}
+
+cudaError_t sort_kmer_matches(const u64* keys, const u64* hashes, u64* keys_out, u64* hashes_out, u64 m, int end_bit,
+                              cudaStream_t s) {
+    size_t temp_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, keys, keys_out, hashes, hashes_out, (long long)m, 0, end_bit, s);
+    void* temp = nullptr;
+    cudaError_t e = cudaMallocAsync(&temp, temp_bytes ? temp_bytes : 16, s);
+    if (e != cudaSuccess) return e;
+    e = cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys, keys_out, hashes, hashes_out, (long long)m, 0, end_bit, s);
+    cudaFreeAsync(temp, s);
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+void launch_match_mark_found(const u64* keys, const u64* hashes, u64 n, const u8* skip, const u64* q, u64 nq, u8* flag,
+                             cudaStream_t s) {
+    if (n == 0 || nq == 0) return;
+    u64 blocks = (n + 255) / 256;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
+    match_mark_found_kernel<<<(unsigned)blocks, 256, 0, s>>>(keys, hashes, n, skip, q, nq, flag); count_launches(1);
+}
+
+void launch_match_num_common(const u64* bh, const u64* boff, const u32* recs, int n, const u64* q, u64 nq, u32 num,
+                             const u8* skip, u8* rec_hit, u8* flag, cudaStream_t s) {
+    if (n <= 0) return;
+    match_num_common_kernel<<<(n + 255) / 256, 256, 0, s>>>(bh, boff, recs, n, q, nq, num, skip, rec_hit, flag); count_launches(1);
 }
 
 // ---------------------------------------------------------------------------------------
