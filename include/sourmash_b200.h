@@ -221,7 +221,7 @@ uint64_t smb_kernel_launches(void);             /* number of kernels launched by
  * bit, so the matrix forms of those formulas call this (host only, no device work). */
 void smb_pow_f64(const double *x, double e, double *out, uintptr_t n);
 void smb_set_profiling(bool on);                /* record CUDA events around the dominant kernels */
-double smb_last_kernel_ms(int32_t which);       /* 0: last pairwise tile kernel, 1: last hash pass */
+double smb_last_kernel_ms(int32_t which);       /* 0: last pairwise tile kernel, 1: last hash pass or combine */
 /* planner of the last all-vs-all count (this thread): {1 = inverted join / 0 = tile kernel,
  * estimated increments, estimated elements, largest hash group seen in the sample} */
 void smb_last_compare_plan(double *out4);
@@ -450,6 +450,20 @@ const uint8_t *smb_kmer_matches_has_invalid(const SmbKmerMatches *m);    /* one 
 uintptr_t smb_kmer_matches_n_found(const SmbKmerMatches *m);
 const uint64_t *smb_kmer_matches_found(const SmbKmerMatches *m);
 void smb_kmer_matches_free(SmbKmerMatches *m);
+
+/* Union, intersection or difference of all rows of a resident set, in one device sort (`sig merge`, `sig intersect`,
+ * `sig subtract`; the reference merges one sketch at a time, minhash.rs:432-516).  Rows must be sorted and unique.
+ * op SMB_COMBINE_UNION: every hash of any row; with abundances, each hash's abundances summed over the rows; num > 0
+ * keeps the first num hashes (what a chain of merges into a num sketch keeps).  SMB_COMBINE_ALL: the hashes of every
+ * row.  SMB_COMBINE_FIRST_ONLY: the hashes of row 0 that no other row holds.  Hashes ascend; abundances (UNION of a
+ * set with abundances only, else null) are parallel to them.  Fails on a set of more than 2^31 - 1 hashes. */
+enum { SMB_COMBINE_UNION = 0, SMB_COMBINE_ALL = 1, SMB_COMBINE_FIRST_ONLY = 2 };
+typedef struct SmbCombined SmbCombined;
+SmbCombined *smb_sketchset_combine(const SmbSketchSet *set, uint32_t op, uint32_t num);
+uintptr_t smb_combined_len(const SmbCombined *c);
+const uint64_t *smb_combined_hashes(const SmbCombined *c);                /* len */
+const uint64_t *smb_combined_abunds(const SmbCombined *c);                /* len, or null */
+void smb_combined_free(SmbCombined *c);
 
 /* Signature objects straight from a sketch set (the tail of _compute_individual,
  * command_sketch.py:770-789): signature g owns rows [g * n_ksizes, (g + 1) * n_ksizes); ksizes

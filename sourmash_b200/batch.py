@@ -343,6 +343,29 @@ def many_vs_many_device(d_hashes_ptr, offsets, db, d_counts_ptr):
              len(offs) - 1, db._ptr, ffi.cast("uint32_t *", int(d_counts_ptr)))
 
 
+COMBINE_OPS = {"union": 0, "all": 1, "first_only": 2}
+
+
+def combine(sset, op, num=0):
+    """Union ("union"), intersection ("all") or difference ("first_only": row 0 minus every other row) of all rows of
+    ``sset`` in one device sort.  Returns ``(hashes, abunds)`` as uint64 arrays in hash order; ``abunds`` holds each
+    hash's summed abundances for a union of a set with abundances, else None.  ``num`` > 0 keeps the union's first
+    ``num`` hashes, as merging into a num sketch does."""
+    code = COMBINE_OPS[op] if isinstance(op, str) else int(op)
+    p = rustcall(lib.smb_sketchset_combine, sset._ptr, code, int(num))
+    try:
+        n = int(lib.smb_combined_len(p))
+        h = np.frombuffer(ffi.buffer(lib.smb_combined_hashes(p), n * 8), dtype=np.uint64).copy() if n else \
+            np.zeros(0, np.uint64)
+        a = None
+        if code == 0 and sset.has_abunds:
+            a = np.frombuffer(ffi.buffer(lib.smb_combined_abunds(p), n * 8), dtype=np.uint64).copy() if n else \
+                np.zeros(0, np.uint64)
+        return h, a
+    finally:
+        lib.smb_combined_free(p)
+
+
 def gather(query, db, threshold=1, max_rounds=None):
     """Iterative min-set-cover; returns (match_ids, intersect_sizes) in pick order."""
     q = _u64(query)

@@ -3130,6 +3130,45 @@ uintptr_t smb_kmer_matches_n_found(const SmbKmerMatches* m) { return m->found.si
 const uint64_t* smb_kmer_matches_found(const SmbKmerMatches* m) { return m->found.data(); }
 void smb_kmer_matches_free(SmbKmerMatches* m) { delete m; }
 
+// `sig merge` / `sig intersect` / `sig subtract` over a resident set (sig/__main__.py:459-712): one device sort of the
+// whole set and one pass over its runs (sketch_combine.cuh); the only readback before the copy-out is the length
+struct SmbCombined {
+    std::vector<uint64_t> hashes, abunds;
+    bool has_abunds = false;
+};
+
+SmbCombined* smb_sketchset_combine(const SmbSketchSet* set, uint32_t op, uint32_t num) {
+    return guarded<SmbCombined*>([&]() -> SmbCombined* {
+        cudaStream_t s = need_gpu();
+        if (op > SMB_COMBINE_FIRST_ONLY) fail(SOURMASH_ERROR_CODE_MSG, "unknown combine op " + std::to_string(op));
+        auto res = std::make_unique<SmbCombined>();
+        res->has_abunds = op == SMB_COMBINE_UNION && set->d_abunds != nullptr;
+        const uint64_t T = set->total();
+        if (T > 0x7fffffffull)
+            fail(SOURMASH_ERROR_CODE_MSG, "set too large to combine (more than 2^31 - 1 hashes)");
+        if (set->n_rows == 0 || T == 0) return res.release();
+        uint64_t *d_h = nullptr, *d_v = nullptr, n = 0;
+        const uint64_t max_key = set_max_key(*set, s);
+        if (t_profiling) t_timer_hash.begin(s);                      // the sort, the run pass, the scan, the scatter
+        CK(smb::sketchset_combine(set->d_hashes, set->d_abunds, set->n_rows, T, set->h_off[1], max_key, op, &d_h, &d_v,
+                                  &n, s));
+        if (t_profiling) t_timer_hash.end(s);
+        DevBuf<uint64_t> out_h, out_v;                                // owned from here on, freed on every path
+        out_h.p = d_h; out_h.n = T; out_h.s = s;
+        out_v.p = d_v; out_v.n = d_v ? T : 0; out_v.s = s;
+        if (op == SMB_COMBINE_UNION && num > 0 && n > num) n = num;   // the bottom num of the union
+        res->hashes.resize(n);
+        out_h.download(res->hashes.data(), n);
+        if (res->has_abunds) { res->abunds.resize(n); out_v.download(res->abunds.data(), n); }
+        sync(s);
+        return res.release();
+    });
+}
+uintptr_t smb_combined_len(const SmbCombined* c) { return c->hashes.size(); }
+const uint64_t* smb_combined_hashes(const SmbCombined* c) { return c->hashes.data(); }
+const uint64_t* smb_combined_abunds(const SmbCombined* c) { return c->has_abunds ? c->abunds.data() : nullptr; }
+void smb_combined_free(SmbCombined* c) { delete c; }
+
 // signatures straight from a sketch set (the tail of _compute_individual, command_sketch.py:770-789):
 // signature s gets rows [s * n_ksizes, (s + 1) * n_ksizes) of `set` as its sketches
 SourmashSignature** smb_signatures_from_sketchset(const SmbSketchSet* set, const uint32_t* ksizes,

@@ -38,6 +38,7 @@
 #include "multigather_kernels.cuh"
 #include "tile_kernels.cuh"
 #include "pair_kernels.cuh"
+#include "sketch_combine.cuh"
 
 namespace smb {
 
@@ -775,6 +776,22 @@ struct DbIndex {
     }
 };
 
+// (hash, payload) pairs stably sorted by hash over the significant bits of max_key: equal hashes keep the order of
+// their payloads.  The payload is the caller's: row ids for the index, element indices for sketchset_combine.
+static cudaError_t sort_hash_pairs(const u64* h, u64* keys_out, const u32* payload, u32* payload_out, u64 T,
+                                   u64 max_key, cudaStream_t s) {
+    const int key_bits = key_bit_length(max_key);
+    size_t bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, bytes, h, keys_out, payload, payload_out, (long long)T, 0, key_bits, s);
+    void* tmp = nullptr;
+    cudaError_t e = cudaMallocAsync(&tmp, bytes ? bytes : 16, s);
+    if (e != cudaSuccess) return e;
+    cub::DeviceRadixSort::SortPairs(tmp, bytes, h, keys_out, payload, payload_out, (long long)T, 0, key_bits, s);
+    cudaFreeAsync(tmp, s);
+    count_launches(1);
+    return cudaGetLastError();
+}
+
 cudaError_t db_index_build(const u64* h, const u64* off, int n, u64 T, u64 max_key, DbIndex** out, cudaStream_t s) {
     *out = nullptr;
     if (n <= 0 || T == 0 || T > 0x7fffffffull) return cudaSuccess;       // CUB's run-length encode counts in int
@@ -790,16 +807,8 @@ cudaError_t db_index_build(const u64* h, const u64* off, int n, u64 T, u64 max_k
     if ((e = cudaMallocAsync(&ix->m_rows, T * sizeof(u32), s)) != cudaSuccess) return e;
     const int blocks = n < SMB_SMS * 16 ? n : SMB_SMS * 16;
     index_rowid_kernel<<<blocks, 256, 0, s>>>(off, n, ids); count_launches(1);
-    {   // (hash, row) pairs sorted by hash where they lie; stable, so rows ascend inside a group
-        const int key_bits = key_bit_length(max_key);
-        size_t bytes = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, bytes, h, keys_sorted, ids, (u32*)ix->m_rows, (long long)T, 0, key_bits, s);
-        void* tmp = nullptr;
-        if ((e = cudaMallocAsync(&tmp, bytes ? bytes : 16, s)) != cudaSuccess) return e;
-        cub::DeviceRadixSort::SortPairs(tmp, bytes, h, keys_sorted, ids, (u32*)ix->m_rows, (long long)T, 0, key_bits, s);
-        cudaFreeAsync(tmp, s);
-        count_launches(1);
-    }
+    // (hash, row) pairs sorted by hash; stable, so rows ascend inside a group
+    if ((e = sort_hash_pairs(h, keys_sorted, ids, (u32*)ix->m_rows, T, max_key, s)) != cudaSuccess) return e;
     // distinct keys + group sizes, then sizes -> offsets
     if ((e = cudaMallocAsync(&ix->m_keys, T * sizeof(u64), s)) != cudaSuccess) return e;
     if ((e = cudaMallocAsync(&ix->m_start, (T + 1) * sizeof(u32), s)) != cudaSuccess) return e;
@@ -839,6 +848,61 @@ cudaError_t db_index_build(const u64* h, const u64* off, int n, u64 T, u64 max_k
 }
 void db_index_destroy(DbIndex* ix) { delete ix; }
 u64 db_index_n_keys(const DbIndex* ix) { return ix->view.n_keys; }
+
+// ------------------------------------------------------------------------------------
+// Union / intersection / difference of all rows of a resident set (sketch_combine.cuh): a stable sort of
+// (hash, element index), one pass over the runs, a scan and a scatter -- five launches and one readback (the output
+// length) whatever the number of rows.
+// ------------------------------------------------------------------------------------
+cudaError_t sketchset_combine(const u64* h, const u64* abund, u64 n_rows, u64 T, u64 row0_end, u64 max_key, u32 op,
+                              u64** out_h, u64** out_v, u64* out_n, cudaStream_t s) {
+    *out_h = *out_v = nullptr;
+    *out_n = 0;
+    if (n_rows == 0 || T == 0) return cudaSuccess;
+    if (T > 0x7fffffffull) return cudaErrorInvalidValue;              // cub's scan counts in int
+    const bool values = abund && op == COMBINE_UNION;
+    JoinScratch scratch(s);
+    cudaError_t e;
+    u32 *idx = nullptr, *idx_sorted = nullptr, *flag = nullptr, *pos = nullptr;
+    u64 *keys = nullptr, *val = nullptr;
+    unsigned long long* d_count = nullptr;
+    if ((e = scratch.alloc((void**)&idx, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&idx_sorted, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&keys, T * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&flag, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&pos, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&d_count, sizeof(unsigned long long))) != cudaSuccess) return e;
+    if (values && (e = scratch.alloc((void**)&val, T * sizeof(u64))) != cudaSuccess) return e;
+    const unsigned blocks = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_SMS * 32);
+    combine_iota_kernel<<<blocks, 256, 0, s>>>(idx, T); count_launches(1);
+    if ((e = sort_hash_pairs(h, keys, idx, idx_sorted, T, max_key, s)) != cudaSuccess) return e;
+    combine_runs_kernel<<<blocks, 256, 0, s>>>(keys, idx_sorted, T, values ? abund : nullptr, op, n_rows, row0_end,
+                                               flag, val);
+    count_launches(1);
+    {
+        size_t bytes = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, bytes, flag, pos, (int)T, s);
+        void* tmp = nullptr;
+        if ((e = cudaMallocAsync(&tmp, bytes ? bytes : 16, s)) != cudaSuccess) return e;
+        cub::DeviceScan::ExclusiveSum(tmp, bytes, flag, pos, (int)T, s);
+        cudaFreeAsync(tmp, s);
+        count_launches(1);
+    }
+    // the output is at most T long: allocated at that bound, so the one readback is the length itself
+    u64 *oh = nullptr, *ov = nullptr;
+    if ((e = cudaMallocAsync((void**)&oh, T * sizeof(u64), s)) != cudaSuccess) return e;
+    if (values && (e = cudaMallocAsync((void**)&ov, T * sizeof(u64), s)) != cudaSuccess) { cudaFreeAsync(oh, s); return e; }
+    combine_scatter_kernel<<<blocks, 256, 0, s>>>(keys, val, flag, pos, T, oh, ov, d_count); count_launches(1);
+    unsigned long long n = 0;
+    cudaMemcpyAsync(&n, d_count, sizeof n, cudaMemcpyDeviceToHost, s);
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
+        cudaFreeAsync(oh, s);
+        if (ov) cudaFreeAsync(ov, s);
+        return e;
+    }
+    *out_h = oh; *out_v = ov; *out_n = n;
+    return cudaSuccess;
+}
 
 void launch_index_count(const DbIndex* ix, const u64* q, u64 nq, u32* counts, cudaStream_t s) {
     if (nq == 0 || ix->view.n_keys == 0) return;

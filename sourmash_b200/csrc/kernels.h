@@ -49,6 +49,16 @@ void launch_index_count(const DbIndex* ix, const uint64_t* q, uint64_t nq, uint3
 void launch_index_count_n(const DbIndex* ix, const uint64_t* q, const uint32_t* d_nq, uint64_t max_nq, uint32_t* counts,
                           cudaStream_t s);
 
+// Union / intersection / difference of all n_rows rows of a resident set (sketch_combine.cuh), in hash order.
+// UNION keeps every hash (with abund: the sum of its abundances in *out_v), ALL the hashes of every row, FIRST_ONLY
+// the hashes of row 0 (elements [0, row0_end)) that no other row holds.  *out_h / *out_v are device arrays the
+// caller frees with cudaFreeAsync (*out_v only for UNION with abund).  cudaErrorInvalidValue: more than 2^31 - 1
+// elements (cub's scan counts in int).
+enum : uint32_t { COMBINE_UNION = 0, COMBINE_ALL = 1, COMBINE_FIRST_ONLY = 2 };
+cudaError_t sketchset_combine(const uint64_t* h, const uint64_t* abund, uint64_t n_rows, uint64_t T, uint64_t row0_end,
+                              uint64_t max_key, uint32_t op, uint64_t** out_h, uint64_t** out_v, uint64_t* out_n,
+                              cudaStream_t s);
+
 // Range-major copy of a resident set and the streaming one-vs-many pass over it (range_kernels.cuh): the key
 // space is cut into P equal ranges, part p of the copy holds every row's elements of range p back to back, CTA p
 // keeps a Bloom bitmap of the query keys of its range in shared memory and streams its part.  range_major_build
