@@ -342,6 +342,15 @@ void smb_one_vs_many(const uint64_t *query, uintptr_t n_query, const SmbSketchSe
 /* the same with the (sorted) query and the n_rows counters in device memory: nothing crosses PCIe */
 void smb_one_vs_many_dev(const uint64_t *d_query, uintptr_t n_query, const SmbSketchSet *db,
                          uint32_t *d_common_out);
+/* Index.search_abund (src/sourmash/index/__init__.py:172-200): the angular similarity (KmerMinHash::angular_similarity,
+ * sketch/minhash.rs:635-680) of one abundance query (sorted-unique hashes q, abundances q_abunds) with every row of a
+ * set that carries abundances, over the hashes <= max_hash of both sides (UINT64_MAX: all of them) -- what
+ * similarity(..., downsample=True) computes after cutting the finer side to the coarser one's max_hash.  scores_out:
+ * n_rows doubles, finalized on the host exactly as kmerminhash_angular_similarity does.  An empty query (or one cut to
+ * nothing) scores 0.0 everywhere; a set without abundances fails with NEEDS_ABUNDANCE_TRACKING, a query that is not
+ * sorted and unique with an error. */
+void smb_search_angular(const SmbSketchSet *db, const uint64_t *q, const uint64_t *q_abunds, uintptr_t nq,
+                        uint64_t max_hash, double *scores_out);
 /* one_vs_many for many queries: counts_out[q * n_rows + r] = |query q ∩ row r| (a Q x n_rows host matrix).
  * q_hashes / q_offsets: the queries as CSR (n_queries + 1 offsets from 0, not decreasing), each sorted and unique.
  * Groups of consecutive queries share one streaming pass over the database (its range-major copy, built on first
@@ -525,6 +534,14 @@ SourmashSignature **smb_sigs_signatures(const SmbSigs *s, const uint32_t *rows, 
  * row (downsample_scaled, sketch/minhash.rs:777-798) */
 SmbSketchSet *smb_sigs_to_sketchset(const SmbSigs *s, const uint32_t *rows, uintptr_t n_rows,
                                     uint64_t max_hash, bool with_abunds);
+/* The subjects of an index held as objects: subject i is the first sketch of sigs[i] when that is not null, else
+ * mhs[i] (either array may be null).  smb_subjects_sketch_info fills sig_index = file = 0; smb_sketchset_from_subjects
+ * puts the subjects' sketches on the device as one set (with_abunds: their abundances too, NEEDS_ABUNDANCE_TRACKING if
+ * one has none), gathered on the host threads straight from the objects. */
+void smb_subjects_sketch_info(const SourmashSignature *const *sigs, const SourmashKmerMinHash *const *mhs, uintptr_t n,
+                              SmbSketchInfo *out);
+SmbSketchSet *smb_sketchset_from_subjects(const SourmashSignature *const *sigs, const SourmashKmerMinHash *const *mhs,
+                                          uintptr_t n, bool with_abunds);
 
 /* reference ABI for .sig I/O: src/core/src/ffi/signature.rs:219-343 (include/sourmash.h:389-414).
  * One SourmashSignature per sketch, filtered by ksize (0: any; compared with the stored ksize)

@@ -314,6 +314,20 @@ def one_vs_many_device(d_query_ptr, n_query, db, d_counts_ptr):
              ffi.cast("uint32_t *", int(d_counts_ptr)))
 
 
+def search_angular(q_hashes, q_abunds, sset, max_hash):
+    """Angular similarity of one abundance query (sorted-unique ``q_hashes``, ``q_abunds``) with every row of ``sset``
+    (which must carry abundances), over the hashes <= ``max_hash`` of both sides: a float64 ``(len(sset),)`` array,
+    bit for bit what ``similarity(..., downsample=True)`` gives for each row when ``max_hash`` is the coarser side's
+    (``2**64 - 1``: every hash)."""
+    q, qa = _u64(q_hashes), _u64(q_abunds)
+    if len(q) != len(qa):
+        raise ValueError("query hashes and abundances differ in length")
+    out = np.zeros(len(sset), dtype=np.float64)
+    rustcall(lib.smb_search_angular, sset._ptr, _ptr(q, "uint64_t *"), _ptr(qa, "uint64_t *"), len(q), int(max_hash),
+             _ptr(out, "double *"))
+    return out
+
+
 def _query_csr(queries):
     "(hashes, offsets) of a list of sorted-unique u64 queries"
     qs = [_u64(q) for q in queries]

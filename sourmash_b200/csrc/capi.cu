@@ -974,6 +974,16 @@ double mh_jaccard(const MH& a, const MH& b) {       // minhash.rs:624-631
     return (double)c.common / (double)std::max<uint64_t>(1, c.usize);
 }
 
+// the tail of minhash.rs:635-680: the score from the dot product and the two sums of squares (u64, wrapped), on the
+// host with libm -- mh_angular and smb_search_angular share it, so the two give the same bits
+double angular_from_terms(uint64_t prod, uint64_t a_sq, uint64_t b_sq) {
+    const double norm_a = std::sqrt((double)a_sq), norm_b = std::sqrt((double)b_sq);
+    if (norm_a == 0. || norm_b == 0.) return 0.0;
+    const double p = std::min((double)prod / (norm_a * norm_b), 1.0);
+    const double distance = 2. * std::acos(p) / 3.14159265358979323846264338327950288;
+    return 1. - distance;
+}
+
 double mh_angular(const MH& a, const MH& b) {       // minhash.rs:635-680
     a.check_compatible(b);
     if (!a.track || !b.track)
@@ -987,11 +997,7 @@ double mh_angular(const MH& a, const MH& b) {       // minhash.rs:635-680
     unsigned long long t[3];
     d_out.download(t, 3);
     sync(s);
-    double norm_a = std::sqrt((double)t[1]), norm_b = std::sqrt((double)t[2]);
-    if (norm_a == 0. || norm_b == 0.) return 0.0;
-    double prod = std::min((double)t[0] / (norm_a * norm_b), 1.0);
-    double distance = 2. * std::acos(prod) / 3.14159265358979323846264338327950288;
-    return 1. - distance;
+    return angular_from_terms(t[0], t[1], t[2]);
 }
 
 double mh_similarity(const MH& a, const MH& b, bool ignore_abundance, bool downsample) {
@@ -2218,6 +2224,58 @@ static void one_vs_many_dev(const uint64_t* d_q, size_t nq, const SmbSketchSet& 
     sync(s);      // q's offsets upload reads a host temporary
 }
 
+// Index.search_abund (index/__init__.py:172-200) over a resident set: every row's angular similarity with one abundance
+// query, elements above max_hash left out on both sides (similarity(..., downsample=True) without a downsampled copy).
+// One device pass (angular_search.cuh) computes the per-row terms; the scores are finalized here with libm.
+void smb_search_angular(const SmbSketchSet* db, const uint64_t* q, const uint64_t* q_abunds, uintptr_t nq,
+                        uint64_t max_hash, double* scores_out) {
+    guarded_void([&] {
+        cudaStream_t s = need_gpu();
+        const size_t n = db->n_rows;
+        for (uintptr_t i = 1; i < nq; ++i)
+            if (q[i] <= q[i - 1]) fail(SOURMASH_ERROR_CODE_MSG, "query hashes are not sorted and unique");
+        if (n == 0) return;
+        // the query cut at max_hash (a prefix) and its own sum of squares
+        const uintptr_t nq_cut = (uintptr_t)(std::upper_bound(q, q + nq, max_hash) - q);
+        uint64_t a_sq = 0;
+        for (uintptr_t i = 0; i < nq_cut; ++i) a_sq += q_abunds[i] * q_abunds[i];
+        if (db->total() == 0 || nq_cut == 0) {            // nothing on one side: every norm or every product is 0
+            if (db->total() && !db->d_abunds)
+                fail(SOURMASH_ERROR_CODE_NEEDS_ABUNDANCE_TRACKING, "sketch needs abundance for this operation");
+            std::fill(scores_out, scores_out + n, 0.0);
+            return;
+        }
+        if (!db->d_abunds)
+            fail(SOURMASH_ERROR_CODE_NEEDS_ABUNDANCE_TRACKING, "sketch needs abundance for this operation");
+        smb::AngularSearchArgs a{};
+        a.q_has_max = q[nq_cut - 1] == UINT64_MAX;
+        a.nq = nq_cut - (a.q_has_max ? 1 : 0);
+        a.q_top = a.nq ? q[a.nq - 1] : 0;
+        a.q_max_abund = a.q_has_max ? q_abunds[nq_cut - 1] : 0;
+        std::vector<uint64_t> chunk(n + 1, 0);
+        for (size_t i = 0; i < n; ++i)
+            chunk[i + 1] = chunk[i] + (db->h_off[i + 1] - db->h_off[i] + smb::ANGULAR_CHUNK - 1) / smb::ANGULAR_CHUNK;
+        DevBuf<uint64_t> d_q(a.nq, s), d_qa(a.nq, s), d_chunk(n + 1, s);
+        d_q.upload(q, a.nq);
+        d_qa.upload(q_abunds, a.nq);
+        d_chunk.upload(chunk.data(), n + 1);
+        DevBuf<unsigned long long> d_prod(n, s), d_bsq(n, s);
+        a.q = d_q.p; a.qa = d_qa.p;
+        a.h = db->d_hashes; a.ab = db->d_abunds; a.off = db->d_off;
+        a.chunk_start = d_chunk.p; a.n_chunks = chunk[n]; a.n_rows = (int)n;
+        a.max_hash = max_hash;
+        a.prod = d_prod.p; a.bsq = d_bsq.p;
+        if (t_profiling) t_timer_hash.begin(s);
+        CK(smb::angular_search(a, s));
+        if (t_profiling) t_timer_hash.end(s);
+        std::vector<unsigned long long> prod(n), bsq(n);
+        d_prod.download(prod.data(), n);
+        d_bsq.download(bsq.data(), n);
+        sync(s);
+        for (size_t i = 0; i < n; ++i) scores_out[i] = angular_from_terms(prod[i], a_sq, bsq[i]);
+    });
+}
+
 uint64_t smb_sketchset_build_index(SmbSketchSet* set) {
     return guarded<uint64_t>([&]() -> uint64_t {
         cudaStream_t s = need_gpu();
@@ -3333,23 +3391,89 @@ SourmashSignature** smb_sigs_signatures(const SmbSigs* s, const uint32_t* rows, 
         return arr;
     });
 }
+// Copies row r of n (src_h[r], src_a[r], off[r + 1] - off[r] elements) into the CSR h / a, rows spread over the host
+// threads: gathering the rows of a large index is a few GB of memcpy
+static void pack_rows(size_t n, const std::vector<uint64_t>& off, const std::vector<const uint64_t*>& src_h,
+                      const std::vector<const uint64_t*>& src_a, uint64_t* h, uint64_t* a) {
+    std::atomic<size_t> next{0};
+    auto worker = [&] {
+        for (;;) {
+            const size_t r0 = next.fetch_add(256);
+            if (r0 >= n) return;
+            for (size_t r = r0; r < std::min(n, r0 + 256); ++r) {
+                const size_t len = off[r + 1] - off[r];
+                if (!len) continue;
+                memcpy(h + off[r], src_h[r], len * 8);
+                if (a) memcpy(a + off[r], src_a[r], len * 8);
+            }
+        }
+    };
+    const size_t nt = std::min<size_t>((size_t)default_threads(), std::max<size_t>(off[n] / (1u << 20), 1));
+    std::vector<std::thread> pool;
+    for (size_t t = 1; t < nt; ++t) pool.emplace_back(worker);
+    worker();
+    for (auto& t : pool) t.join();
+}
+
 SmbSketchSet* smb_sigs_to_sketchset(const SmbSigs* s, const uint32_t* rows, uintptr_t n_rows, uint64_t max_hash,
                                     bool with_abunds) {
     return guarded<SmbSketchSet*>([&]() -> SmbSketchSet* {
         const smb::SigBatch& B = s->b;
         const size_t n = rows ? n_rows : B.sketches.size();
-        std::vector<uint64_t> off(n + 1, 0), h, ab;
+        std::vector<uint64_t> off(n + 1, 0);
+        std::vector<const uint64_t*> src_h(n), src_a(n);
         for (size_t r = 0; r < n; ++r) {
             const size_t i = rows ? rows[r] : r;
             if (i >= B.sketches.size()) fail(SOURMASH_ERROR_CODE_INTERNAL, "sketch row out of range");
             const uint64_t* b = B.mins.data() + B.off[i];
             const uint64_t* e = B.mins.data() + B.off[i + 1];
             if (max_hash) e = std::upper_bound(b, e, max_hash);        // downsample_scaled == prefix
-            h.insert(h.end(), b, e);
-            if (with_abunds) ab.insert(ab.end(), B.abunds.data() + B.off[i], B.abunds.data() + B.off[i] + (e - b));
-            off[r + 1] = h.size();
+            src_h[r] = b; src_a[r] = B.abunds.data() + B.off[i];
+            off[r + 1] = off[r] + (uint64_t)(e - b);
         }
-        return smb_sketchset_from_host(h.data(), off.data(), n, with_abunds ? ab.data() : nullptr);
+        std::unique_ptr<uint64_t[]> h(new uint64_t[std::max<uint64_t>(off[n], 1)]);
+        std::unique_ptr<uint64_t[]> ab(with_abunds ? new uint64_t[std::max<uint64_t>(off[n], 1)] : nullptr);
+        pack_rows(n, off, src_h, src_a, h.get(), ab.get());
+        return smb_sketchset_from_host(h.get(), off.data(), n, ab.get());
+    });
+}
+
+// The first sketch of subject i of a search: the signature sigs[i] when it is not null, else the sketch mhs[i]
+static const MH& subject_sketch(const SourmashSignature* const* sigs, const SourmashKmerMinHash* const* mhs, size_t i) {
+    if (sigs && sigs[i]) {
+        if (sigs[i]->sketches.empty()) fail(SOURMASH_ERROR_CODE_INTERNAL, "internal error: \"found unsupported sketch type\"");
+        return sigs[i]->sketches[0];
+    }
+    if (!mhs || !mhs[i]) fail(SOURMASH_ERROR_CODE_INTERNAL, "subject " + std::to_string(i) + " has no sketch");
+    return *mhs[i];
+}
+void smb_subjects_sketch_info(const SourmashSignature* const* sigs, const SourmashKmerMinHash* const* mhs, uintptr_t n,
+                              SmbSketchInfo* out) {
+    guarded_void([&] {
+        for (uintptr_t i = 0; i < n; ++i) {
+            const MH& m = subject_sketch(sigs, mhs, i);
+            out[i] = SmbSketchInfo{};
+            out[i].ksize = m.ksize; out[i].num = m.num; out[i].max_hash = m.max_hash; out[i].seed = m.seed;
+            out[i].hash_function = (uint32_t)m.hash_function; out[i].has_abund = m.track; out[i].n_mins = m.mins.size();
+        }
+    });
+}
+SmbSketchSet* smb_sketchset_from_subjects(const SourmashSignature* const* sigs, const SourmashKmerMinHash* const* mhs,
+                                          uintptr_t n, bool with_abunds) {
+    return guarded<SmbSketchSet*>([&]() -> SmbSketchSet* {
+        std::vector<uint64_t> off(n + 1, 0);
+        std::vector<const uint64_t*> src_h(n), src_a(n);
+        for (uintptr_t i = 0; i < n; ++i) {
+            const MH& m = subject_sketch(sigs, mhs, i);
+            if (with_abunds && !m.track)
+                fail(SOURMASH_ERROR_CODE_NEEDS_ABUNDANCE_TRACKING, "sketch needs abundance for this operation");
+            src_h[i] = m.mins.data(); src_a[i] = m.abunds.data();
+            off[i + 1] = off[i] + m.mins.size();
+        }
+        std::unique_ptr<uint64_t[]> h(new uint64_t[std::max<uint64_t>(off[n], 1)]);
+        std::unique_ptr<uint64_t[]> ab(with_abunds ? new uint64_t[std::max<uint64_t>(off[n], 1)] : nullptr);
+        pack_rows(n, off, src_h, src_a, h.get(), ab.get());
+        return smb_sketchset_from_host(h.get(), off.data(), n, ab.get());
     });
 }
 

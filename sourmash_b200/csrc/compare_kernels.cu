@@ -39,6 +39,7 @@
 #include "tile_kernels.cuh"
 #include "pair_kernels.cuh"
 #include "sketch_combine.cuh"
+#include "angular_search.cuh"
 
 namespace smb {
 
@@ -902,6 +903,48 @@ cudaError_t sketchset_combine(const u64* h, const u64* abund, u64 n_rows, u64 T,
     }
     *out_h = oh; *out_v = ov; *out_n = n;
     return cudaSuccess;
+}
+
+// ------------------------------------------------------------------------------------
+// One abundance query against every row of a set with abundances (angular_search.cuh): with the global directory's
+// three builder launches and the bitmap, at most five launches whatever the number of rows; no readback.
+// ------------------------------------------------------------------------------------
+cudaError_t angular_search(AngularSearchArgs a, cudaStream_t s) {
+    if (a.n_rows <= 0) return cudaSuccess;
+    cudaError_t e;
+    if ((e = cudaMemsetAsync(a.prod, 0, (size_t)a.n_rows * sizeof(unsigned long long), s)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(a.bsq, 0, (size_t)a.n_rows * sizeof(unsigned long long), s)) != cudaSuccess) return e;
+    if (a.n_chunks == 0) return cudaSuccess;
+    JoinScratch scratch(s);
+    a.split = a.nq <= ANGULAR_SPLIT_MAX ? 1 : 0;
+    if (a.split) {
+        const u64 entries = a.nq > 256 ? a.nq : 256;                     // about one key per bucket
+        u32 sh = 0;
+        while (sh < 63 && (a.q_top >> sh) >= entries) ++sh;
+        a.shift = sh; a.nb = (a.q_top >> sh) + 1;
+    } else {
+        int nb_log2 = 12;                                                // as one_vs_many_dev
+        while (nb_log2 < 26 && (1ull << nb_log2) < 2 * a.nq) ++nb_log2;
+        u32 sh = 0;
+        while (sh < 63 && (a.q_top >> sh) >= (1ull << nb_log2)) ++sh;
+        a.shift = sh; a.nb = (a.q_top >> sh) + 1;
+        a.fine_log2 = 3;
+        u32 *dir = nullptr, *bm = nullptr;
+        const size_t bm_words = ((size_t)a.nb << a.fine_log2) / 32 + 2;
+        if ((e = scratch.alloc((void**)&dir, (a.nb + 2) * sizeof(u32))) != cudaSuccess) return e;
+        if ((e = scratch.alloc((void**)&bm, bm_words * sizeof(u32))) != cudaSuccess) return e;
+        if ((e = cudaMemsetAsync(bm, 0, bm_words * sizeof(u32), s)) != cudaSuccess) return e;
+        launch_build_global_dir(a.q, a.nq, (int)sh, a.nb, dir, s);
+        launch_build_query_bitmap(a.q, a.nq, (int)sh, a.fine_log2, bm, s);
+        a.gdir = dir; a.bitmap = bm;
+    }
+    const size_t smem = a.split ? angular_split_smem(a.nq, a.nb) : 0;
+    cudaFuncSetAttribute(angular_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    const u64 ctas_per_sm = smem + 1024 <= (size_t)110 * 1024 ? 2 : 1;   // two CTAs of 512 threads fill an SM
+    u64 blocks = (a.n_chunks + ANGULAR_THREADS / 32 - 1) / (ANGULAR_THREADS / 32);   // one chunk per warp at most
+    if (blocks > (u64)SMB_SMS * ctas_per_sm) blocks = (u64)SMB_SMS * ctas_per_sm;
+    angular_search_kernel<<<(unsigned)blocks, ANGULAR_THREADS, smem, s>>>(a); count_launches(1);
+    return cudaGetLastError();
 }
 
 void launch_index_count(const DbIndex* ix, const u64* q, u64 nq, u32* counts, cudaStream_t s) {

@@ -327,6 +327,34 @@ void launch_match_num_common(const uint64_t* bh, const uint64_t* boff, const uin
                              uint64_t nq, uint32_t num, const uint8_t* skip, uint8_t* rec_hit, uint8_t* flag,
                              cudaStream_t s);
 
+// Angular search (angular_search.cuh): for one abundance query and every row r of a set with abundances, over the
+// elements <= max_hash of both, prod[r] = sum of q_abund * s_abund over shared hashes and bsq[r] = sum of s_abund^2
+// (u64, wrapping).  The caller fills the query and subject fields; angular_search plans the probe layout, builds the
+// global directory when the query is too large for the split table, zeroes prod / bsq and launches.
+static constexpr uint64_t ANGULAR_CHUNK = 1024;        // elements of a row per warp task
+// Queries up to this many keys become the shared-memory split table: 8 bytes per key plus a directory of about one u16
+// entry per key is at most 164 KB, inside a CTA's 227 KB.  The table format itself stops at 32 759 keys, which would
+// need 262 KB of keys alone.
+static constexpr uint64_t ANGULAR_SPLIT_MAX = 16382;
+struct AngularSearchArgs {
+    // query, cut at max_hash, sorted-unique, without a trailing UINT64_MAX
+    const uint64_t* q; const uint64_t* qa;
+    uint64_t nq, q_top;                 // q_top = q[nq - 1] (0 when nq == 0)
+    int q_has_max;                      // the query holds UINT64_MAX (max_hash == UINT64_MAX) ...
+    uint64_t q_max_abund;               // ... with this abundance
+    // probe layout (filled by angular_search)
+    int split;                          // 1: shared-memory split table; 0: global directory + occupancy bitmap
+    uint32_t shift; uint64_t nb;        // bucket = key >> shift, buckets [0, nb)
+    const uint32_t* gdir; const uint32_t* bitmap; int fine_log2;
+    // subjects
+    const uint64_t* h; const uint64_t* ab; const uint64_t* off;
+    const uint64_t* chunk_start;        // [n_rows + 1] prefix of ceil(row length / ANGULAR_CHUNK)
+    uint64_t n_chunks; int n_rows;
+    uint64_t max_hash;
+    unsigned long long* prod; unsigned long long* bsq;   // [n_rows]
+};
+cudaError_t angular_search(AngularSearchArgs a, cudaStream_t s);
+
 // kernel-launch accounting (smb_kernel_launches)
 void count_launches(int n);
 

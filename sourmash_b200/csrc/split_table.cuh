@@ -86,4 +86,15 @@ __host__ __device__ __forceinline__ u32 split_probe_rest(const SplitTable& t, u6
     }
 }
 
+// position of q in the table, -1 when absent: the fast path's directory entry and low words reject most misses, a
+// possible hit or a crowded bucket walks the bucket from its start (the sentinels end the walk)
+__host__ __device__ __forceinline__ int split_probe_find(const SplitTable& t, u64 q, u32 shift) {
+    u32 ent = 0;
+    if (!split_probe_low(t, q, shift, ent) && !(ent & 1u)) return -1;
+    for (u32 p = (ent & 0xfffeu) >> 1;; ++p) {
+        const u64 k = ((u64)t.hi[p] << 32) | t.lo[p];
+        if (k >= q) return k == q ? (int)p : -1;
+    }
+}
+
 }  // namespace smb

@@ -13,6 +13,7 @@ from . import batch as B
 from .manifest import CollectionManifest, _check_select_parameters
 from .minhash import flatten_and_intersect_scaled
 from .search import calc_threshold_from_bp, make_containment_query, make_jaccard_search_query
+from .sigset import _INFO_DTYPE
 
 IndexSearchResult = namedtuple("IndexSearchResult", "score, signature, location")
 GatherResult = namedtuple("GatherResult", "match, intersect_size, containment, location")
@@ -42,6 +43,32 @@ def select_signature(ss, *, ksize=None, moltype=None, scaled=0, num=0, containme
     return True
 
 
+_U64_MAX = 2**64 - 1
+_HASH_FUNCTION = {"DNA": 1, "protein": 2, "dayhoff": 3, "hp": 4}
+
+
+def _abi_scaled(max_hash):
+    "KmerMinHash::scaled() of the library (sketch/minhash.rs:233-235): the scaled similarity(downsample=True) compares"
+    if not max_hash:
+        return 0
+    v = float(2**64) / float(max_hash)
+    return _U64_MAX if v >= float(2**64) else int(v)
+
+
+def _angular_cut(q_max_hash, s_max_hash):
+    """The max_hash both sketches are cut at by `similarity(other, downsample=True)` (sketch/minhash.rs:682-702), or None
+    when that call fails the scaled check of angular_similarity.  Equal scaled: no cut (num sketches of any num too).
+    Else the finer side is downsampled to the coarser one's scaled, and its max_hash must then equal the coarser one's."""
+    sq, ss = _abi_scaled(q_max_hash), _abi_scaled(s_max_hash)
+    if sq == ss:
+        return _U64_MAX if q_max_hash == s_max_hash else None
+    coarse_max_hash, fine_scaled = (q_max_hash, ss) if sq > ss else (s_max_hash, sq)
+    if fine_scaled == 0:                                  # a num sketch is not downsampled: num vs scaled
+        return None
+    cut = B.max_hash_for_scaled(max(sq, ss))
+    return cut if cut == coarse_max_hash else None
+
+
 class LinearIndex:
     "A list of signatures searched on the GPU (reference: LinearIndex, index/__init__.py:380-470)."
 
@@ -52,6 +79,8 @@ class LinearIndex:
         self._signatures = list(_signatures) if _signatures else []
         self.filename = filename
         self._device = None          # (scaled -> (SketchSet, sizes)) cache
+        self._abund_cols = None      # search_abund: metadata of the subjects ...
+        self._abund_device = None    # ... and their groups with abundances on the device
 
     @property
     def location(self):
@@ -72,7 +101,7 @@ class LinearIndex:
 
     def insert(self, node):
         self._signatures.append(node)
-        self._device = None
+        self._device = self._abund_cols = self._abund_device = None
 
     def save(self, path):
         from .signature import save_signatures_to_json
@@ -246,23 +275,99 @@ class LinearIndex:
                                 counted.get(i), cache))
                 for i, query in enumerate(queries)]
 
+    # -- search_abund: the subjects' metadata, their resident groups with abundances, the match objects ------------
+    def _subject_ptrs(self, positions):
+        """The library's view of the subjects at ``positions``: (signature pointers, sketch pointers, objects to keep
+        alive).  A SourmashSignature is passed as it is; any other subject by its ``.minhash``, as the reference's loop
+        only reads ``subject.minhash``."""
+        from ._lowlevel import ffi
+        from .signature import SourmashSignature
+        sigs, mhs, keep = [], [], []
+        for i in positions:
+            o = self._signatures[i]
+            if isinstance(o, SourmashSignature):
+                sigs.append(o._get_objptr())
+                mhs.append(ffi.NULL)
+            else:
+                mh = o.minhash
+                keep.append(mh)
+                sigs.append(ffi.NULL)
+                mhs.append(mh._get_objptr())
+        return ffi.new("SourmashSignature *[]", sigs), ffi.new("SourmashKmerMinHash *[]", mhs), keep
+
+    def _abund_info(self):
+        """ksize (as stored), hash_function, seed, max_hash and has_abund of every subject, in index order (one
+        library call, no sketch copied; built once)"""
+        if self._abund_cols is None:
+            from ._ffi import rustcall
+            from ._lowlevel import ffi, lib
+            n = len(self._signatures)
+            sigs, mhs, _keep = self._subject_ptrs(range(n))
+            info = ffi.new("SmbSketchInfo[]", max(n, 1))
+            rustcall(lib.smb_subjects_sketch_info, sigs, mhs, n, info)
+            self._abund_cols = np.frombuffer(ffi.buffer(info, n * ffi.sizeof("SmbSketchInfo")), dtype=_INFO_DTYPE).copy()
+        return self._abund_cols
+
+    def _abund_sketchset(self, positions):
+        "the subjects at ``positions`` as one resident set with abundances, gathered straight from the objects"
+        from ._ffi import rustcall
+        from ._lowlevel import lib
+        sigs, mhs, _keep = self._subject_ptrs(positions)
+        return B.SketchSet(rustcall(lib.smb_sketchset_from_subjects, sigs, mhs, len(positions), True))
+
+    def _subjects(self, positions):
+        "the subject objects at ``positions``"
+        return [self._signatures[i] for i in positions]
+
+    def _abund_groups(self):
+        """Subjects grouped by their max_hash: {max_hash: (positions, SketchSet with abundances)}, one upload per group
+        (built once, beside the flat ``_groups()``)."""
+        if self._abund_device is None:
+            groups = {}
+            for pos, mx in enumerate(self._abund_info()["max_hash"].tolist()):
+                groups.setdefault(mx, []).append(pos)
+            self._abund_device = {mx: (np.array(pos), self._abund_sketchset(pos)) for mx, pos in groups.items()}
+        return self._abund_device
+
     def search_abund(self, query, *, threshold=None, **kwargs):
-        """Matches by angular similarity of abundance sketches, best first (Index.search_abund, index/__init__.py:172-200):
-        one `similarity(..., downsample=True)` per subject, as there."""
-        if not query.minhash.track_abundance:
+        """Matches by angular similarity of abundance sketches, best first (Index.search_abund, index/__init__.py:172-200).
+
+        The reference calls `query.similarity(subject, downsample=True)` subject by subject.  Here every resident group
+        (one max_hash) is scored in one device pass (batch.search_angular), both sides cut at the max_hash that call
+        downsamples to.  The first subject at which the reference's loop raises is found from the metadata, and raises
+        the same exception before anything is scored; signature objects are built for the matches only."""
+        query_mh = query.minhash
+        if not query_mh.track_abundance:
             raise TypeError("'search_abund' requires query signature with abundance information")
         if threshold is None:
             raise TypeError("'search_abund' requires 'threshold'")
         threshold = float(threshold)
-        matches = []
-        for subj, loc in self.signatures_with_location():
-            if not subj.minhash.track_abundance:
+        info = self._abund_info()
+        if not len(info):
+            return []
+        track, max_hash = info["has_abund"].astype(bool), info["max_hash"]
+        mq = query_mh._max_hash
+        cuts = {mx: _angular_cut(mq, mx) for mx in np.unique(max_hash).tolist()}
+        # check_compatible (sketch/minhash.rs:886-912) on the stored columns: ksize as stored (3k for protein-family
+        # sketches), hash function, seed; the max_hash condition is in `cuts`
+        hf = _HASH_FUNCTION[query_mh.moltype]
+        bad = ~track | (info["ksize"] != query_mh.ksize * (1 if hf == 1 else 3)) | (info["hash_function"] != hf)
+        bad |= info["seed"] != np.uint64(query_mh.seed)
+        bad |= np.isin(max_hash, np.array([mx for mx, c in cuts.items() if c is None], dtype=np.uint64))
+        if bad.any():
+            i = int(np.argmax(bad))
+            if not track[i]:
                 raise TypeError("'search_abund' requires subject signatures with abundance information")
-            score = query.similarity(subj, downsample=True)
-            if score >= threshold:
-                matches.append(IndexSearchResult(score, subj, loc))
-        matches.sort(key=lambda x: -x.score)
-        return matches
+            query.similarity(self._subjects([i])[0], downsample=True)   # raises the reference's exception for this subject
+            raise AssertionError("subject %d was expected to be incompatible with the query" % i)
+        qh, qa = query_mh._mins_array(), query_mh._abunds_array()
+        scores = np.empty(len(info), dtype=np.float64)
+        for mx, (pos, sset) in self._abund_groups().items():
+            scores[pos] = B.search_angular(qh, qa, sset, cuts[mx])
+        order = np.argsort(-scores, kind="stable")              # list.sort(key=-score) is stable: ties keep index order
+        keep = order[scores[order] >= threshold].tolist()
+        return [IndexSearchResult(float(scores[i]), subj, self.location)
+                for i, subj in zip(keep, self._subjects(keep))]
 
     def search(self, query, *, threshold=None, do_containment=False, do_max_containment=False,
                best_only=False, **kwargs):
@@ -317,6 +422,7 @@ class ZipFileLinearIndex(LinearIndex):
         self.use_manifest = use_manifest
         self.filename = storage.path
         self._device = None
+        self._abund_device = None
         self._objects = {}
         self._sigset = _sigset if _sigset is not None else SignatureSet.from_files(
             [storage.path], use_manifest=use_manifest, traverse_yield_all=traverse_yield_all)
@@ -443,6 +549,24 @@ class ZipFileLinearIndex(LinearIndex):
             k = int(ss.ksize[row])
             out.append((k if mol == "DNA" else k // 3, mol, int(ss.seed[row])))   # protein-family sketches store 3*k
         return out
+
+    def _abund_info(self):
+        ss = self._sigset
+        info = np.zeros(len(self._rows), dtype=_INFO_DTYPE)
+        for name in ("ksize", "hash_function", "seed", "max_hash", "has_abund"):
+            info[name] = getattr(ss, name)[self._rows]
+        return info
+
+    def _abund_sketchset(self, positions):
+        return self._sigset.to_sketchset(self._rows[positions], with_abunds=True)
+
+    def _subjects(self, positions):
+        "the signature objects at ``positions``, the ones not built yet in one call"
+        missing = sorted({i for i in positions if i not in self._objects})
+        if missing:
+            for i, obj in zip(missing, self._sigset.signatures(self._rows[missing])):
+                self._objects[i] = obj
+        return [self._objects[i] for i in positions]
 
     def _groups(self):
         "Selected rows grouped by scaled (or num), each group one CSR upload straight from the parser's arrays."
