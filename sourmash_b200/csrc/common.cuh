@@ -13,6 +13,10 @@ typedef uint8_t u8;
 // Number of SMs on an H100 SXM; grids for persistent-style kernels are sized in multiples of it.
 #define SMB_SMS 132
 
+// L2 cache of the devices the library is built for (sm_90a: H100 SXM / PCIe, H200, GH200 all have 50 MB); sizes
+// the windows that keep scattered writes L2-resident.
+#define SMB_L2_BYTES (50ull * 1024 * 1024)
+
 // Shared memory of kernels that tests/host_emul/simt.h also runs on the CPU (SMB_SIMT_EMUL: one CTA at a
 // time as cooperative fibers, so block-shared storage is plain static storage there).
 #ifdef SMB_SIMT_EMUL

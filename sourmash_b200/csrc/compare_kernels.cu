@@ -635,7 +635,11 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
         *out = guard.release();
         return cudaSuccess;
     }
-    u32 *key_a = nullptr, *key_b = nullptr, *eblk = nullptr, *d_count = nullptr;
+    // windows of pos[] for the position pass (SMB_STRIPE_POS_WINDOW, a number of elements, overrides the L2 rule for tests)
+    const char* pw = getenv("SMB_STRIPE_POS_WINDOW");
+    const int pos_lg = stripe_pos_window_log2(SMB_L2_BYTES, pw ? strtoull(pw, nullptr, 10) : 0ull, T_all);
+    const u32 nw = (u32)(((T_all - 1) >> pos_lg) + 1);
+    u32 *key_a = nullptr, *key_b = nullptr, *eblk = nullptr, *d_count = nullptr, *boff = nullptr;
     u64 *pay_a = nullptr, *pay_b = nullptr;
     if ((e = scratch.alloc((void**)&key_a, Tp * 2 * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&pay_a, Tp * 2 * sizeof(u64))) != cudaSuccess) return e;
@@ -643,6 +647,7 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     const u64 nblk = (T_all >> STRIPE_EBLK_LOG2) + 1;
     if ((e = scratch.alloc((void**)&eblk, (nblk + 1) * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&d_count, 16)) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&boff, (2 * (size_t)nw + 1) * sizeof(u32))) != cudaSuccess) return e;   // offsets | cursors
     const unsigned grid = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_SMS * 32);
     const int low_bits = stripe_low_bits(max_key);
     // 1. 32-bit sort keys (top bits of the hashes) + payloads (low bits, element index)
@@ -662,14 +667,34 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     if ((e = scratch.alloc(&d_sort, sort_bytes)) != cudaSuccess) return e;
     cub::DeviceRadixSort::SortPairs(d_sort, sort_bytes, key_a, key_b, pay_a, pay_b, (long long)T, 0, key_bits, s);
     count_launches(1);
-    // 3. tags + inverse permutation.  Runs of equal keys that hold more than one hash are noticed on the way (key_a is
-    //    free: worklist) and redone in order, one warp per run (pay_a is free: the ordered payloads of those runs)
+    // 3. tags + inverse permutation: the tag kernel appends (element, position) pairs to the buckets of the pos[]
+    //    windows (pay_a is free: 8 B per element), the window pass writes pos[] from them; when pos[] is one window it
+    //    stays in L2 as a whole and the tag kernel stores it directly.  Runs of equal keys that hold more than one hash
+    //    are noticed on the way (key_a is free: worklist) and redone in order after the window pass, one warp per run
+    //    (pay_a is free again: the ordered payloads of those runs)
     u32* worklist = low_bits ? key_a : nullptr;
     if (low_bits) cudaMemsetAsync(d_count, 0, sizeof(u32), s);
     stripe_eblk_kernel<<<(unsigned)std::min<u64>((nblk + 255) / 256, (u64)SMB_SMS * 8), 256, 0, s>>>(off, n, T_all, eblk);
-    if (js->tag16) stripe_tag_kernel<u16><<<grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u16*)js->tags, js->pos, worklist, d_count, js->swz);
-    else stripe_tag_kernel<u32><<<grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u32*)js->tags, js->pos, worklist, d_count, js->swz);
-    count_launches(2);
+    count_launches(1);
+    const bool windows = nw > 1;
+    u64* bucket = windows ? pay_a : nullptr;
+    if (windows) {
+        stripe_window_offsets_kernel<<<(nw + 256) / 256, 256, 0, s>>>(off, n, js->ebeg, js->eend, js->sharded ? d_doff : off, T_all, T,
+                                                                      pos_lg, nw, boff, boff + nw + 1);
+        count_launches(1);
+    }
+    const unsigned tag_grid = (unsigned)std::min<u64>((T + STRIPE_TAG_TILE - 1) / STRIPE_TAG_TILE, (u64)SMB_SMS * 16);
+    if (js->tag16)
+        stripe_tag_kernel<u16><<<tag_grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u16*)js->tags, js->pos, worklist, d_count, js->swz,
+                                                        bucket, boff + nw + 1, pos_lg, nw);
+    else
+        stripe_tag_kernel<u32><<<tag_grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u32*)js->tags, js->pos, worklist, d_count, js->swz,
+                                                        bucket, boff + nw + 1, pos_lg, nw);
+    count_launches(1);
+    if (windows) {
+        stripe_pos_window_kernel<<<(unsigned)((T + 256 * STRIPE_POS_UNROLL - 1) / (256 * STRIPE_POS_UNROLL)), 256, 0, s>>>(pay_a, T, js->pos);
+        count_launches(1);
+    }
     if (low_bits) {
         if (js->tag16) stripe_fix_kernel<u16><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u16*)js->tags, js->pos, js->swz);
         else stripe_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz);

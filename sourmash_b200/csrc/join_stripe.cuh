@@ -30,8 +30,9 @@
 namespace smb {
 
 static constexpr int STRIPE_EBLK_LOG2 = 11;           // element blocks of the row lookup table: 25 000 entries for 5e7 elements, so
-                                                      // the table and the row offsets it leads to stay in L1 (the tag kernel is bound
-                                                      // by L2 transactions: its scattered 4-byte writes of pos[] are enough of those)
+                                                      // the table and the row offsets it leads to stay in L1 (the tag kernel's
+                                                      // chain of dependent loads payload -> block table -> row offsets hits L1)
+static constexpr int STRIPE_MAX_WINDOWS = 2048;       // pos[] windows of the position pass (shared counters of the tag kernel)
 static constexpr int STRIPE_MAX_ROWS = 32;            // rows per CTA (upper bound)
 static constexpr int STRIPE_HEADER = 544;             // bytes in front of the counters: s_beg[32] + s_end[32] + control words, 16-aligned
 static constexpr int STRIPE_TAG_PAD = 128;            // head flags stored behind the end of the tag stream
@@ -109,9 +110,10 @@ __global__ void __launch_bounds__(256) stripe_sizes_kernel(const u64* __restrict
 // run appends the run's head to a worklist (the list can hold every element, so it never overflows), and
 // stripe_fix_kernel redoes the tags and positions of the listed runs -- one warp per run: the payloads are
 // ranked against each other (they are distinct: they end in the element index) and written in order to `tmp`
-// (the sort's input buffer, free by now; a run uses the slots of its own stream positions), then the run's
-// tags and positions are derived from the ordered payloads.  Ascending payloads = ascending (low bits, element)
-// = groups contiguous, rows ascending.
+// (the sort's input buffer, which held the position buckets and is free again once stripe_pos_window_kernel has
+// run; a run uses the slots of its own stream positions), then the run's tags and positions are derived from the
+// ordered payloads -- after the position pass, whose positions of these runs they overwrite.  Ascending payloads =
+// ascending (low bits, element) = groups contiguous, rows ascending.
 __device__ __forceinline__ void stripe_note_descent(const u32* __restrict__ key32s, const u64* __restrict__ pays, u64 q, u32 k,
                                                     u32* __restrict__ worklist, u32* __restrict__ d_count) {
     u64 p = q - 1;                                        // q: a descent (same key as q - 1, smaller payload).  Any earlier one in this run?
@@ -122,23 +124,78 @@ __device__ __forceinline__ void stripe_note_descent(const u32* __restrict__ key3
     worklist[atomicAdd(d_count, 1u)] = (u32)p;            // p = head of the run
 }
 
-// sorted (key, payload) stream -> tags (row | head flag) and the inverse permutation.  Four stream positions per
-// thread, their loads issued together: the kernel is a chain of dependent loads (payload -> block table -> row
-// offsets) and is bound by latency, not by bytes.
+// ---- the inverse permutation pos[e] = q, written window by window ------------------------------------------
+// Stored directly, pos[e] = q is one 4-byte write per element to a random place of a T_all x 4 B array (200 MB for
+// the benchmark's 5e7 elements, four times the L2): nearly every write lands on a sector that is not resident and
+// costs a partial-sector write to HBM.  Instead the tag kernel appends (e << 32 | q) to the bucket of e's window of
+// pos[] (2^lg elements, a slice that fits the L2 several times over), and stripe_pos_window_kernel writes the
+// buckets out in window order: each window's lines are written while they stay in L2 and leave it whole, once.
+// Every element of the stream occurs once, so the size of every bucket is known before the tag kernel runs, the
+// order inside a bucket does not matter, and pos[] is the same whatever order the CTAs append in.
+
+// log2 of the window: the largest power of two with 4 B x window <= L2 / 3 (so that the window, the bucket stream
+// passing through and the tags being written share the L2), or `requested` (a power of two, rounded down; 0 = the
+// rule); raised until the T_all elements span at most STRIPE_MAX_WINDOWS windows
+__host__ __device__ __forceinline__ int stripe_pos_window_log2(u64 l2_bytes, u64 requested, u64 T_all) {
+    int lg = 0;
+    if (requested) while ((2ull << lg) <= requested) ++lg;
+    else while ((12ull << (lg + 1)) <= l2_bytes) ++lg;
+    while (T_all && ((T_all - 1) >> lg) >= (u64)STRIPE_MAX_WINDOWS) ++lg;
+    return lg < 31 ? lg : 31;                             // elements are u32
+}
+
+// bucket offsets: boff[w] = number of stream elements e < w << lg, for w = 0 .. nw (boff[nw] = T), and the
+// append cursors cur[w] = boff[w].  The stream holds the elements [ebeg[r], eend[r]) of every row r (whole rows, or
+// a key-range shard's slices), doff[r] of them in rows < r; the rows' CSR ranges off[] ascend, so the count below
+// x is doff[r] + the part of row r's range below x, for the row r whose CSR range holds x.
+__global__ void __launch_bounds__(256) stripe_window_offsets_kernel(const u64* __restrict__ off, int n, const u64* __restrict__ ebeg,
+                                                                   const u64* __restrict__ eend, const u64* __restrict__ doff,
+                                                                   u64 T_all, u64 T, int lg, u32 nw, u32* __restrict__ boff,
+                                                                   u32* __restrict__ cur) {
+    for (u32 w = blockIdx.x * blockDim.x + threadIdx.x; w <= nw; w += gridDim.x * blockDim.x) {
+        const u64 x = (u64)w << lg;
+        u64 below = T;
+        if (x < T_all) {
+            const u32 r = stripe_row_of(off, n, x);
+            const u64 b = ebeg[r], len = eend[r] - b;
+            below = doff[r] + (x > b ? (x - b < len ? x - b : len) : 0);
+        }
+        boff[w] = (u32)below;
+        if (w < nw) cur[w] = (u32)below;
+    }
+}
+
+// sorted (key, payload) stream -> tags (row | head flag), and the (element, position) pairs of the inverse
+// permutation appended to the buckets of their pos[] windows.  A CTA takes tiles of U x blockDim consecutive stream
+// positions; per tile each element takes a rank in its window from a shared counter, one atomicAdd per (tile,
+// window) on the window's cursor reserves the tile's run of the bucket, and the elements are written into it.
+// Without buckets (null `bucket`: pos[] is a single window, T_all <= 2^lg) pos[e] = q is stored here -- the whole
+// array stays in L2, so the store costs what the window pass's would, without the 8 B per element of buckets.
+// U positions per thread, their loads issued together: the chain of dependent loads (payload -> block table -> row
+// offsets) hits L1 and is bound by latency; the tags and buckets are written in order.
+static constexpr int STRIPE_TAG_U = 8;                // stream positions per thread and tile (tiles of 2048 at 256 threads)
+static constexpr int STRIPE_TAG_TILE = STRIPE_TAG_U * 256;
 template <typename TagT>
 __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__ key32s, const u64* __restrict__ pays,
                                                         const u64* __restrict__ off, const u32* __restrict__ eblk, u64 T,
-                                                        TagT* __restrict__ tags, u32* __restrict__ pos,
-                                                        u32* __restrict__ worklist, u32* __restrict__ d_count, u32 swz) {
-    constexpr int U = 4;
-    const u64 stride = (u64)gridDim.x * blockDim.x;
-    for (u64 q0 = (u64)blockIdx.x * blockDim.x + threadIdx.x; q0 < T; q0 += stride * U) {
+                                                        TagT* __restrict__ tags, u32* __restrict__ pos, u32* __restrict__ worklist,
+                                                        u32* __restrict__ d_count, u32 swz, u64* __restrict__ bucket = nullptr,
+                                                        u32* __restrict__ cur = nullptr, int lg = 0, u32 nw = 0) {
+    constexpr int U = STRIPE_TAG_U;
+    SMB_SHARED u32 s_cnt[STRIPE_MAX_WINDOWS];             // elements of the tile per window, then ...
+    SMB_SHARED u32 s_base[STRIPE_MAX_WINDOWS];            // ... where the tile's run of each bucket starts
+    const u64 tile = (u64)U * blockDim.x;
+    for (u64 t0 = (u64)blockIdx.x * tile; t0 < T; t0 += (u64)gridDim.x * tile) {
+        if (bucket) {
+            for (u32 w = threadIdx.x; w < nw; w += blockDim.x) s_cnt[w] = 0;
+            __syncthreads();
+        }
         u64 p[U], pp[U];
-        u32 k[U], kp[U], r[U];
+        u32 k[U], kp[U], r[U], rk[U];
         u64 nx[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const u64 q = q0 + (u64)u * stride;
+            const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
             const bool in = q < T;
             p[u] = in ? pays[q] : 0;
             k[u] = in ? key32s[q] : 0;
@@ -151,22 +208,54 @@ __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__
         for (int u = 0; u < U; ++u) nx[u] = off[r[u] + 1];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const u64 q = q0 + (u64)u * stride;
+            const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
             if (q >= T) continue;
             const u32 e = (u32)p[u];
             const bool head = q == 0 || k[u] != kp[u] || (p[u] >> 32) != (pp[u] >> 32);
             u32 rr = r[u];
             u64 end = nx[u];
-            while (end <= (u64)e) end = off[++rr + 1];    // e < T = off[n]: stops at the owning row, empty rows skipped
+            while (end <= (u64)e) end = off[++rr + 1];    // e < T_all = off[n]: stops at the owning row, empty rows skipped
             tags[q] = (TagT)(stripe_col(rr, swz) | (head ? StripeTag<TagT>::HEAD : 0u));
-            pos[e] = (u32)q;
+            if (bucket) rk[u] = atomicAdd(&s_cnt[e >> lg], 1u);
+            else pos[e] = (u32)q;                         // one window: all of pos[] stays in L2
             // a run that mixes hashes (null worklist: the keys hold every bit, no such runs)
             if (worklist && q && k[u] == kp[u] && p[u] < pp[u]) stripe_note_descent(key32s, pays, q, k[u], worklist, d_count);
+        }
+        if (!bucket) continue;                            // uniform: a kernel parameter
+        __syncthreads();
+        for (u32 w = threadIdx.x; w < nw; w += blockDim.x) {
+            const u32 c = s_cnt[w];
+            if (c) s_base[w] = atomicAdd(cur + w, c);
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
+            if (q >= T) continue;
+            const u32 e = (u32)p[u];
+            bucket[s_base[e >> lg] + rk[u]] = ((u64)e << 32) | q;
         }
     }
     // STRIPE_TAG_PAD head flags behind the end: the count kernel reads ahead of a group without bounds checks
     const u64 gt = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (gt < (u64)STRIPE_TAG_PAD) tags[T + gt] = (TagT)StripeTag<TagT>::HEAD;
+}
+
+// the buckets in window order -> pos[e] = q.  Each block takes STRIPE_POS_PER_BLOCK consecutive pairs and blocks
+// start in index order, so the resident blocks work on one or two windows of pos[] at a time; the pairs are read once
+// (evict-first: they must not push the window out of the L2).
+static constexpr int STRIPE_POS_UNROLL = 4;
+__global__ void __launch_bounds__(256) stripe_pos_window_kernel(const u64* __restrict__ bucket, u64 T, u32* __restrict__ pos) {
+    const u64 i0 = (u64)blockIdx.x * blockDim.x * STRIPE_POS_UNROLL + threadIdx.x;
+    u64 v[STRIPE_POS_UNROLL];
+#pragma unroll
+    for (int u = 0; u < STRIPE_POS_UNROLL; ++u) {
+        const u64 i = i0 + (u64)u * blockDim.x;
+        v[u] = i < T ? ld_stream_u64(bucket + i) : ~0ull;
+    }
+#pragma unroll
+    for (int u = 0; u < STRIPE_POS_UNROLL; ++u)
+        if (v[u] != ~0ull) pos[v[u] >> 32] = (u32)v[u];
 }
 
 // the listed runs again, in order (see stripe_note_descent)
