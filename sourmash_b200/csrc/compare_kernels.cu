@@ -522,9 +522,11 @@ cudaError_t join_estimate(const u64* h, const u64* off, int n, u64 max_key, unsi
 // ------------------------------------------------------------------------------------
 struct JoinStripe {
     cudaStream_t stream = 0;
-    void* mem = nullptr;      // tags + pos + sizes (+ the slice ranges of a key-range shard)
+    void* mem = nullptr;      // tags + pos + sizes + order + sel (+ the slice ranges of a key-range shard)
     void* tags = nullptr;
     u32 *pos = nullptr, *sizes = nullptr;
+    u32* order = nullptr;     // the rows in the order they are counted: ascending label (stripe_label_kernel), row inside a label
+    u32* sel = nullptr;       // sel[row_begin, row_end): the rows of a launch over that range, in `order`'s order
     const u64 *ebeg = nullptr, *eend = nullptr;
     u64 T = 0;                // elements in the stream (all of the set, or one key range of it)
     int n = 0, rows_per_block = 0, upper_only = 1, tag16 = 0, sharded = 0;
@@ -551,6 +553,28 @@ static cudaError_t stripe_set_smem() {
     if ((e = stripe_set_smem_one<TagT, false, 1>()) != cudaSuccess) return e;
     if ((e = stripe_set_smem_one<TagT, true, 2>()) != cudaSuccess) return e;
     return stripe_set_smem_one<TagT, false, 2>();
+}
+
+// js->order from the finished stream: one label per row, then a stable sort of the rows by label (rows ascending
+// inside a label; a set with no shared hashes keeps the identity order)
+static cudaError_t stripe_make_order(JoinStripe* js, JoinScratch& scratch, cudaStream_t s) {
+    const int n = js->n;
+    u32* lab = nullptr;
+    cudaError_t e;
+    if ((e = scratch.alloc((void**)&lab, 3 * (size_t)n * sizeof(u32))) != cudaSuccess) return e;
+    u32 *lab_out = lab + n, *rowid = lab_out + n;
+    const unsigned grid = (unsigned)std::min((n + 7) / 8, SMB_SMS * 8);       // one warp per row
+    if (js->tag16) stripe_label_kernel<u16><<<grid, 256, 0, s>>>((const u16*)js->tags, js->pos, js->ebeg, js->eend, n, js->swz, lab, rowid);
+    else stripe_label_kernel<u32><<<grid, 256, 0, s>>>((const u32*)js->tags, js->pos, js->ebeg, js->eend, n, js->swz, lab, rowid);
+    count_launches(1);
+    const int bits = key_bit_length((u64)n);
+    size_t sort_bytes = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, lab, lab_out, rowid, js->order, n, 0, bits, s);
+    void* d_sort = nullptr;
+    if ((e = scratch.alloc(&d_sort, sort_bytes)) != cudaSuccess) return e;
+    cub::DeviceRadixSort::SortPairs(d_sort, sort_bytes, lab, lab_out, rowid, js->order, n, 0, bits, s);
+    count_launches(1);
+    return cudaGetLastError();
 }
 
 // *out stays null (with cudaSuccess) when the layout does not apply: 2^32 - 256 or more elements, or a row of n
@@ -613,15 +637,17 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     const size_t Tp = (size_t)((T + 63) & ~63ull);
     const size_t Tall_p = (size_t)((T_all + 63) & ~63ull);
     const size_t Tt = Tp + STRIPE_TAG_PAD;                          // the tag stream + its padding of head flags
-    // tags | pos (indexed by CSR element: the whole set's size) | sizes | slice ranges of a shard
-    if ((e = cudaMallocAsync(&js->mem, (Tt + Tall_p + np) * sizeof(u32) + (js->sharded ? 2 * np * sizeof(u64) : 0), s)) != cudaSuccess)
+    // tags | pos (indexed by CSR element: the whole set's size) | sizes | order | sel | slice ranges of a shard
+    if ((e = cudaMallocAsync(&js->mem, (Tt + Tall_p + 3 * np) * sizeof(u32) + (js->sharded ? 2 * np * sizeof(u64) : 0), s)) != cudaSuccess)
         return e;
     js->tags = js->mem;
     js->pos = (u32*)js->mem + Tt;
     js->sizes = js->pos + Tall_p;
+    js->order = js->sizes + np;
+    js->sel = js->order + np;
     stripe_sizes_kernel<<<(n + 255) / 256, 256, 0, s>>>(off, n, js->sizes); count_launches(1);
     if (js->sharded) {
-        u64* eb = (u64*)(js->sizes + np);
+        u64* eb = (u64*)(js->sel + np);
         stripe_slice_ranges_kernel<<<(n + 255) / 256, 256, 0, s>>>(off, d_beg, d_cnt, n, eb, eb + np); count_launches(1);
         js->ebeg = eb; js->eend = eb + np;
     } else {
@@ -631,7 +657,7 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
         if (js->tag16) stripe_tag_kernel<u16><<<1, 256, 0, s>>>(nullptr, nullptr, off, nullptr, 0, (u16*)js->tags, js->pos, nullptr, nullptr, 0u);
         else stripe_tag_kernel<u32><<<1, 256, 0, s>>>(nullptr, nullptr, off, nullptr, 0, (u32*)js->tags, js->pos, nullptr, nullptr, 0u);
         count_launches(1);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if ((e = stripe_make_order(js, scratch, s)) != cudaSuccess) return e;
         *out = guard.release();
         return cudaSuccess;
     }
@@ -700,7 +726,7 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
         else stripe_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz);
         count_launches(1);
     }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = stripe_make_order(js, scratch, s)) != cudaSuccess) return e;
     *out = guard.release();
     return cudaSuccess;
 }
@@ -711,8 +737,15 @@ cudaError_t join_stripe_create(const u64* h, const u64* off, int n, u64 T, u64 m
 static cudaError_t stripe_launch(const JoinStripe* js, int row_begin, int row_end, double* d_out, u32* d_counts, u16* d_counts16,
                                  cudaStream_t s) {
     if (row_end <= row_begin) return cudaSuccess;
+    const u32* rows = js->order;                                    // the whole set: the order itself
+    if (row_end - row_begin < js->n) {
+        rows = js->sel + row_begin;                                 // the callers' ranges do not overlap, so no launch
+                                                                    // overwrites the rows of one still in flight
+        stripe_select_rows_kernel<<<1, 1024, 0, s>>>(js->order, js->n, row_begin, row_end, js->sel + row_begin);
+        count_launches(1);
+    }
     StripeArgs a{js->tags, js->pos, js->ebeg, js->eend, js->sizes, js->T, js->n, js->rows_per_block, row_begin, row_end, d_out,
-                 d_counts, d_counts16, js->swz};
+                 d_counts, d_counts16, js->swz, rows};
     const int blocks = (row_end - row_begin + js->rows_per_block - 1) / js->rows_per_block;
     const bool upper = js->upper_only;
     const bool two = js->ctas_per_sm == 2;

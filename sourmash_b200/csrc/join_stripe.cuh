@@ -295,6 +295,84 @@ __global__ void __launch_bounds__(128) stripe_fix_kernel(const u32* __restrict__
     }
 }
 
+// ---- which rows are counted together -----------------------------------------------------------------------
+// The count kernel's reads of a group's tags hit the L2 when other rows of the same wave of CTAs have just read them.
+// In index order a wave (two rows per CTA, two CTAs per SM: 528 rows) holds a few members of every family of related
+// sketches, so each shared group is fetched from HBM again in every wave.  Rows are therefore counted in the order
+// of a label that related rows share: label[r] = min(r, the lowest row of the group of each of r's first
+// STRIPE_LABEL_GROUPS elements that are not singletons, among its first STRIPE_LABEL_SCAN).  Rows ascend inside a group, so a group's lowest row is the
+// row of its head tag (stripe_col undone: it is an involution on whole 32-column blocks).  One warp per row; an
+// element at stream position q is a singleton when q and q + 1 both hold head flags (the padding makes q + 1 safe);
+// the walk back to the head reads 32 tags per ballot and ends at position 0 at the latest, which is always a head.
+// Only a row's first STRIPE_LABEL_SCAN elements are looked at: where rows share few hashes, scanning whole rows for 8
+// shared elements reads the whole stream (0.36 ms on 10 000 rows of 5 000 hashes that share none), for an order that
+// gains nothing there.  rowid[r] = r: the values of the stable sort by label that makes the order.
+static constexpr int STRIPE_LABEL_GROUPS = 8;
+static constexpr int STRIPE_LABEL_SCAN = 256;
+template <typename TagT>
+__global__ void __launch_bounds__(256) stripe_label_kernel(const TagT* __restrict__ tags, const u32* __restrict__ pos,
+                                                          const u64* __restrict__ ebeg, const u64* __restrict__ eend, int n, u32 swz,
+                                                          u32* __restrict__ label, u32* __restrict__ rowid) {
+    constexpr u32 HEAD = StripeTag<TagT>::HEAD;
+    const u32 lane = lane_id();
+    const u32 warps = gridDim.x * (blockDim.x >> 5);
+    for (u32 r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < (u32)n; r += warps) {
+        u32 best = r;
+        int left = STRIPE_LABEL_GROUPS;
+        const u64 beg = ebeg[r], end = min(eend[r], beg + STRIPE_LABEL_SCAN);
+        for (u64 e0 = beg; e0 < end && left > 0; e0 += 32) {
+            const u64 e = e0 + lane;
+            u32 q = 0;
+            bool shared = false;
+            if (e < end) {
+                q = pos[e];
+                shared = !(((u32)tags[q] & HEAD) && ((u32)tags[(size_t)q + 1] & HEAD));
+            }
+            u32 m = __ballot_sync(0xffffffffu, shared);
+            for (; m && left > 0; m &= m - 1, --left) {
+                const u32 qj = __shfl_sync(0xffffffffu, q, __ffs(m) - 1);
+                for (u32 base = qj;; base -= 32) {
+                    const bool valid = base >= lane;
+                    const u32 t = valid ? (u32)tags[base - lane] : 0u;
+                    const u32 h = __ballot_sync(0xffffffffu, valid && (t & HEAD));
+                    if (h) {
+                        const u32 head = __shfl_sync(0xffffffffu, t, __ffs(h) - 1) & (HEAD - 1u);
+                        best = min(best, stripe_col(head, swz));
+                        break;
+                    }
+                }
+            }
+        }
+        if (lane == 0) { label[r] = best; rowid[r] = r; }
+    }
+}
+
+// the rows of `order` that lie in [row_begin, row_end), in the order they have there: the slot order of a launch over
+// a range of rows.  One CTA.
+__global__ void __launch_bounds__(1024) stripe_select_rows_kernel(const u32* __restrict__ order, int n, int row_begin, int row_end,
+                                                                 u32* __restrict__ out) {
+    SMB_SHARED u32 s_warp[33];                            // per warp: rows selected, then where its rows go; [32] total
+    const u32 lane = lane_id(), w = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    u32 base = 0;
+    for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+        const int i = i0 + (int)threadIdx.x;
+        const u32 r = i < n ? order[i] : 0xffffffffu;
+        const bool in = r >= (u32)row_begin && r < (u32)row_end;
+        const u32 m = __ballot_sync(0xffffffffu, in);
+        if (lane == 0) s_warp[w] = __popc(m);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            u32 run = 0;
+            for (u32 k = 0; k < nwarps; ++k) { const u32 c = s_warp[k]; s_warp[k] = run; run += c; }
+            s_warp[32] = run;
+        }
+        __syncthreads();
+        if (in) out[base + s_warp[w] + __popc(m & ((1u << lane) - 1u))] = r;
+        base += s_warp[32];
+        __syncthreads();
+    }
+}
+
 // ---- the count kernel -------------------------------------------------------------------------------------
 struct StripeArgs {
     const void* tags;        // u16 or u32 (template parameter of the kernel)
@@ -308,7 +386,13 @@ struct StripeArgs {
     u32* out_counts;         // raw counters of the rows instead (a key-range shard's partial counts), same layout
     u16* out_counts16;       // ... as 16-bit counters (rows shorter than 65 536 hashes: half the bytes to exchange)
     u32 swz;                 // the tags hold stripe_col(row, swz)
+    const u32* rows;         // the rows of [row_begin, row_end) in slot order: CTA b counts rows[b * rows_per_block + i]
+                             //   (null: index order, slot i counts row row_begin + i)
 };
+
+__host__ __device__ __forceinline__ u32 stripe_slot_row(const StripeArgs& a, int slot) {
+    return a.rows ? a.rows[slot] : (u32)(a.row_begin + slot);
+}
 
 // A counter of the stripe is bumped through the 32-bit shared-memory address of its row: one address add and one
 // ATOMS per increment.  (atomicAdd on the generic pointer made the compiler rebuild the shared-window base --
@@ -326,8 +410,9 @@ __device__ __forceinline__ void stripe_inc_if(StripeRowRef row, u32 col, bool on
 }
 #endif
 
-// One CTA = rows [r0, r1) of the result.  Work items are (row, chunk of 32 consecutive elements), handed to the
-// warps chunk index first, so that all rows of the CTA -- and, as CTAs start together, all CTAs of a wave --
+// One CTA = the rows of rows_per_block consecutive slots of a.rows (rows sharing a label sit in neighbouring slots, so
+// a wave of CTAs reads the same groups and they stay in L2; see stripe_label_kernel).  Work items are (row, chunk of 32
+// consecutive elements), handed to the warps chunk index first, so that all rows of the CTA -- and, as CTAs start together, all CTAs of a wave --
 // move through the hash-ordered stream together.  For every element with a successor in its group the warp
 // reads the 32 tags behind it (two elements' reads in flight), and 32 more while no group head has turned up; the
 // lanes in front of the next group head increment their counters.  UPPER: only later members (= higher rows) are counted, i.e. the cells (i, j > i);
@@ -342,11 +427,13 @@ __global__ void __launch_bounds__(1024, CTAS) join_stripe_kernel(StripeArgs a) {
     u32* s_ctl = reinterpret_cast<u32*>(stripe_smem + 2 * STRIPE_MAX_ROWS * sizeof(u64));   // [0] next item, [1] chunks of the longest row
     u32* stripe = reinterpret_cast<u32*>(stripe_smem + STRIPE_HEADER);      // [rows][n]
     const TagT* __restrict__ tags = reinterpret_cast<const TagT*>(a.tags);
-    const int r0 = a.row_begin + (int)blockIdx.x * a.rows_per_block;
-    const int r1 = min(a.row_end, r0 + a.rows_per_block);
-    const int rows = r1 - r0;
+    const int s0 = (int)blockIdx.x * a.rows_per_block;
+    const int rows = min(a.row_end - a.row_begin - s0, a.rows_per_block);
     const u32 n = (u32)a.n;
-    for (u32 i = threadIdx.x; i < (u32)rows; i += blockDim.x) { s_beg[i] = a.ebeg[r0 + i]; s_end[i] = a.eend[r0 + i]; }
+    for (u32 i = threadIdx.x; i < (u32)rows; i += blockDim.x) {
+        const u32 row = stripe_slot_row(a, s0 + (int)i);
+        s_beg[i] = a.ebeg[row]; s_end[i] = a.eend[row];
+    }
     if (threadIdx.x == 0) { s_ctl[0] = 0; s_ctl[1] = 0; }
     for (u32 i = threadIdx.x; i < (u32)rows * n; i += blockDim.x) stripe[i] = 0;
     __syncthreads();
@@ -435,7 +522,7 @@ __global__ void __launch_bounds__(1024, CTAS) join_stripe_kernel(StripeArgs a) {
     __syncthreads();
     // counts -> float64 rows, written once (streaming stores: the matrix is not read again by this kernel)
     for (int al = 0; al < rows; ++al) {
-        const int row = r0 + al;
+        const int row = (int)stripe_slot_row(a, s0 + al);
         const u32* __restrict__ srow = stripe + (size_t)al * n;
         if (a.out_counts) {                                // a shard of the keys: partial counts, summed over the shards later
             u32* __restrict__ crow = a.out_counts + (size_t)(row - a.row_begin) * n;
