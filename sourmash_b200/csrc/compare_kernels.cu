@@ -527,6 +527,7 @@ struct JoinStripe {
     u32 *pos = nullptr, *sizes = nullptr;
     u32* order = nullptr;     // the rows in the order they are counted: ascending label (stripe_label_kernel), row inside a label
     u32* sel = nullptr;       // sel[row_begin, row_end): the rows of a launch over that range, in `order`'s order
+    u32* succ = nullptr;      // successor bit of every CSR element (stripe_tag_kernel): the count kernel's test for later members
     const u64 *ebeg = nullptr, *eend = nullptr;
     u64 T = 0;                // elements in the stream (all of the set, or one key range of it)
     int n = 0, rows_per_block = 0, upper_only = 1, tag16 = 0, sharded = 0;
@@ -637,23 +638,27 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     const size_t Tp = (size_t)((T + 63) & ~63ull);
     const size_t Tall_p = (size_t)((T_all + 63) & ~63ull);
     const size_t Tt = Tp + STRIPE_TAG_PAD;                          // the tag stream + its padding of head flags
-    // tags | pos (indexed by CSR element: the whole set's size) | sizes | order | sel | slice ranges of a shard
-    if ((e = cudaMallocAsync(&js->mem, (Tt + Tall_p + 3 * np) * sizeof(u32) + (js->sharded ? 2 * np * sizeof(u64) : 0), s)) != cudaSuccess)
+    const size_t succ_words = Tall_p / 32;                          // even: the slice ranges behind stay 8-byte aligned
+    // tags | pos (indexed by CSR element: the whole set's size) | sizes | order | sel | succ (ditto) | slice ranges of a shard
+    if ((e = cudaMallocAsync(&js->mem, (Tt + Tall_p + 3 * np + succ_words) * sizeof(u32) + (js->sharded ? 2 * np * sizeof(u64) : 0), s)) !=
+        cudaSuccess)
         return e;
     js->tags = js->mem;
     js->pos = (u32*)js->mem + Tt;
     js->sizes = js->pos + Tall_p;
     js->order = js->sizes + np;
     js->sel = js->order + np;
+    js->succ = js->sel + np;
     stripe_sizes_kernel<<<(n + 255) / 256, 256, 0, s>>>(off, n, js->sizes); count_launches(1);
     if (js->sharded) {
-        u64* eb = (u64*)(js->sel + np);
+        u64* eb = (u64*)(js->succ + succ_words);
         stripe_slice_ranges_kernel<<<(n + 255) / 256, 256, 0, s>>>(off, d_beg, d_cnt, n, eb, eb + np); count_launches(1);
         js->ebeg = eb; js->eend = eb + np;
     } else {
         js->ebeg = off; js->eend = off + 1;
     }
     if (T == 0) {                                                   // no hash in this key range: every partial count is zero
+        cudaMemsetAsync(js->succ, 0, succ_words * sizeof(u32), s);
         if (js->tag16) stripe_tag_kernel<u16><<<1, 256, 0, s>>>(nullptr, nullptr, off, nullptr, 0, (u16*)js->tags, js->pos, nullptr, nullptr, 0u);
         else stripe_tag_kernel<u32><<<1, 256, 0, s>>>(nullptr, nullptr, off, nullptr, 0, (u32*)js->tags, js->pos, nullptr, nullptr, 0u);
         count_launches(1);
@@ -661,11 +666,15 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
         *out = guard.release();
         return cudaSuccess;
     }
-    // windows of pos[] for the position pass (SMB_STRIPE_POS_WINDOW, a number of elements, overrides the L2 rule for tests)
+    // windows and sub-windows of pos[] for the position pass (SMB_STRIPE_POS_WINDOW and SMB_STRIPE_POS_SUBWINDOW, numbers
+    // of elements, override the rules for tests)
     const char* pw = getenv("SMB_STRIPE_POS_WINDOW");
-    const int pos_lg = stripe_pos_window_log2(SMB_L2_BYTES, pw ? strtoull(pw, nullptr, 10) : 0ull, T_all);
+    const char* psw = getenv("SMB_STRIPE_POS_SUBWINDOW");
+    int pos_lg = 0, sub_lg = 0;
+    stripe_pos_levels(SMB_L2_BYTES, pw ? strtoull(pw, nullptr, 10) : 0ull, psw ? strtoull(psw, nullptr, 10) : 0ull, T_all, pos_lg, sub_lg);
     const u32 nw = (u32)(((T_all - 1) >> pos_lg) + 1);
-    u32 *key_a = nullptr, *key_b = nullptr, *eblk = nullptr, *d_count = nullptr, *boff = nullptr;
+    const u32 nsub = (u32)(((T_all - 1) >> sub_lg) + 1);
+    u32 *key_a = nullptr, *key_b = nullptr, *eblk = nullptr, *d_count = nullptr, *boff = nullptr, *sboff = nullptr;
     u64 *pay_a = nullptr, *pay_b = nullptr;
     if ((e = scratch.alloc((void**)&key_a, Tp * 2 * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&pay_a, Tp * 2 * sizeof(u64))) != cudaSuccess) return e;
@@ -674,6 +683,7 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     if ((e = scratch.alloc((void**)&eblk, (nblk + 1) * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&d_count, 16)) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&boff, (2 * (size_t)nw + 1) * sizeof(u32))) != cudaSuccess) return e;   // offsets | cursors
+    if ((e = scratch.alloc((void**)&sboff, (2 * (size_t)nsub + 1) * sizeof(u32))) != cudaSuccess) return e;  // ... of the sub-windows
     const unsigned grid = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_SMS * 32);
     const int low_bits = stripe_low_bits(max_key);
     // 1. 32-bit sort keys (top bits of the hashes) + payloads (low bits, element index)
@@ -693,10 +703,12 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     if ((e = scratch.alloc(&d_sort, sort_bytes)) != cudaSuccess) return e;
     cub::DeviceRadixSort::SortPairs(d_sort, sort_bytes, key_a, key_b, pay_a, pay_b, (long long)T, 0, key_bits, s);
     count_launches(1);
-    // 3. tags + inverse permutation: the tag kernel appends (element, position) pairs to the buckets of the pos[]
-    //    windows (pay_a is free: 8 B per element), the window pass writes pos[] from them; when pos[] is one window it
-    //    stays in L2 as a whole and the tag kernel stores it directly.  Runs of equal keys that hold more than one hash
-    //    are noticed on the way (key_a is free: worklist) and redone in order after the window pass, one warp per run
+    // 3. tags + inverse permutation + successor bits: the tag kernel appends (element, position, bit) entries to the
+    //    buckets of the pos[] windows (pay_a is free: 8 B per element), the partition splits them into the buckets of
+    //    the sub-windows (the sort's temporary storage is free: it holds the keys' and payloads' second buffers), and
+    //    the sub-window pass writes pos[] and succ from shared memory; when pos[] is one window it stays in L2 as a whole
+    //    and the tag kernel stores positions and bits directly.  Runs of equal keys that hold more than one hash are
+    //    noticed on the way (key_a is free: worklist) and redone in order after the position pass, one warp per run
     //    (pay_a is free again: the ordered payloads of those runs)
     u32* worklist = low_bits ? key_a : nullptr;
     if (low_bits) cudaMemsetAsync(d_count, 0, sizeof(u32), s);
@@ -704,26 +716,47 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     count_launches(1);
     const bool windows = nw > 1;
     u64* bucket = windows ? pay_a : nullptr;
+    const u64* doff = js->sharded ? d_doff : off;
     if (windows) {
-        stripe_window_offsets_kernel<<<(nw + 256) / 256, 256, 0, s>>>(off, n, js->ebeg, js->eend, js->sharded ? d_doff : off, T_all, T,
-                                                                      pos_lg, nw, boff, boff + nw + 1);
-        count_launches(1);
+        stripe_window_offsets_kernel<<<(nw + 256) / 256, 256, 0, s>>>(off, n, js->ebeg, js->eend, doff, T_all, T, pos_lg, nw, boff, boff + nw + 1);
+        stripe_window_offsets_kernel<<<(nsub + 256) / 256, 256, 0, s>>>(off, n, js->ebeg, js->eend, doff, T_all, T, sub_lg, nsub, sboff,
+                                                                        sboff + nsub + 1);
+        count_launches(2);
+    } else {
+        cudaMemsetAsync(js->succ, 0, succ_words * sizeof(u32), s);  // the tag kernel sets the bits
     }
     const unsigned tag_grid = (unsigned)std::min<u64>((T + STRIPE_TAG_TILE - 1) / STRIPE_TAG_TILE, (u64)SMB_SMS * 16);
     if (js->tag16)
         stripe_tag_kernel<u16><<<tag_grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u16*)js->tags, js->pos, worklist, d_count, js->swz,
-                                                        bucket, boff + nw + 1, pos_lg, nw);
+                                                        bucket, boff + nw + 1, pos_lg, nw, js->succ);
     else
         stripe_tag_kernel<u32><<<tag_grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u32*)js->tags, js->pos, worklist, d_count, js->swz,
-                                                        bucket, boff + nw + 1, pos_lg, nw);
+                                                        bucket, boff + nw + 1, pos_lg, nw, js->succ);
     count_launches(1);
     if (windows) {
-        stripe_pos_window_kernel<<<(unsigned)((T + 256 * STRIPE_POS_UNROLL - 1) / (256 * STRIPE_POS_UNROLL)), 256, 0, s>>>(pay_a, T, js->pos);
-        count_launches(1);
+        u64* sub = (u64*)d_sort;
+        if (sort_bytes < T * sizeof(u64) && (e = scratch.alloc((void**)&sub, T * sizeof(u64))) != cudaSuccess) return e;
+        const u64 chunks = std::min<u64>(((1ull << pos_lg) + STRIPE_SUB_TILE - 1) / STRIPE_SUB_TILE, 1024);
+        const size_t part_smem = (size_t)STRIPE_SUB_TILE * sizeof(u64);
+        if ((e = cudaFuncSetAttribute(stripe_sub_partition_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)part_smem)) != cudaSuccess)
+            return e;
+        stripe_sub_partition_kernel<<<dim3((unsigned)chunks, nw), STRIPE_SUB_THREADS, part_smem, s>>>(pay_a, boff, pos_lg, sub_lg, sboff + nsub + 1,
+                                                                                                       sub);
+        const size_t sub_smem = ((size_t)4 << sub_lg) + ((size_t)1 << sub_lg) / 8;
+        if ((e = cudaFuncSetAttribute(stripe_pos_sub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sub_smem)) != cudaSuccess) return e;
+        if ((e = cudaFuncSetAttribute(stripe_pos_sub_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)) !=
+            cudaSuccess)
+            return e;
+        stripe_pos_sub_kernel<<<nsub, STRIPE_SUB_THREADS, sub_smem, s>>>(sub, sboff, T_all, sub_lg, js->pos, js->succ);
+        count_launches(2);
     }
     if (low_bits) {
-        if (js->tag16) stripe_fix_kernel<u16><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u16*)js->tags, js->pos, js->swz);
-        else stripe_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz);
+        if (js->tag16)
+            stripe_fix_kernel<u16><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u16*)js->tags, js->pos, js->swz,
+                                                               js->succ);
+        else
+            stripe_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz,
+                                                               js->succ);
         count_launches(1);
     }
     if ((e = stripe_make_order(js, scratch, s)) != cudaSuccess) return e;
@@ -745,7 +778,7 @@ static cudaError_t stripe_launch(const JoinStripe* js, int row_begin, int row_en
         count_launches(1);
     }
     StripeArgs a{js->tags, js->pos, js->ebeg, js->eend, js->sizes, js->T, js->n, js->rows_per_block, row_begin, row_end, d_out,
-                 d_counts, d_counts16, js->swz, rows};
+                 d_counts, d_counts16, js->swz, rows, js->succ};
     const int blocks = (row_end - row_begin + js->rows_per_block - 1) / js->rows_per_block;
     const bool upper = js->upper_only;
     const bool two = js->ctas_per_sm == 2;

@@ -165,6 +165,13 @@ __global__ void __launch_bounds__(256) stripe_window_offsets_kernel(const u64* _
     }
 }
 
+// The successor bit succ[e] (bit e & 31 of word e >> 5, one bit per CSR element of the whole set): 1 when the stream
+// position behind e's holds the same hash, i.e. e has a later member in its group.  The count kernel reads it instead
+// of the tag behind each element (a random 2-byte read of the 100 MB stream per element); it is decided here, where
+// the neighbours of q are loaded anyway, travels in bit 63 of the element's bucket entry, and is written with pos[]
+// by stripe_pos_sub_kernel (or by atomicOr here, when pos[] is one window).  With `succ`, a bucket entry holds the
+// element relative to its window: succ << 63 | (e mod 2^lg) << 32 | q (lg <= 31).
+
 // sorted (key, payload) stream -> tags (row | head flag), and the (element, position) pairs of the inverse
 // permutation appended to the buckets of their pos[] windows.  A CTA takes tiles of U x blockDim consecutive stream
 // positions; per tile each element takes a rank in its window from a shared counter, one atomicAdd per (tile,
@@ -180,11 +187,13 @@ __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__
                                                         const u64* __restrict__ off, const u32* __restrict__ eblk, u64 T,
                                                         TagT* __restrict__ tags, u32* __restrict__ pos, u32* __restrict__ worklist,
                                                         u32* __restrict__ d_count, u32 swz, u64* __restrict__ bucket = nullptr,
-                                                        u32* __restrict__ cur = nullptr, int lg = 0, u32 nw = 0) {
+                                                        u32* __restrict__ cur = nullptr, int lg = 0, u32 nw = 0,
+                                                        u32* __restrict__ succ = nullptr) {
     constexpr int U = STRIPE_TAG_U;
     SMB_SHARED u32 s_cnt[STRIPE_MAX_WINDOWS];             // elements of the tile per window, then ...
     SMB_SHARED u32 s_base[STRIPE_MAX_WINDOWS];            // ... where the tile's run of each bucket starts
     const u64 tile = (u64)U * blockDim.x;
+    const u64 wmask = (1ull << lg) - 1ull;
     for (u64 t0 = (u64)blockIdx.x * tile; t0 < T; t0 += (u64)gridDim.x * tile) {
         if (bucket) {
             for (u32 w = threadIdx.x; w < nw; w += blockDim.x) s_cnt[w] = 0;
@@ -193,6 +202,7 @@ __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__
         u64 p[U], pp[U];
         u32 k[U], kp[U], r[U], rk[U];
         u64 nx[U];
+        u32 scm = 0;                                      // bit u: the successor bit (succ) of position u
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
@@ -216,8 +226,14 @@ __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__
             u64 end = nx[u];
             while (end <= (u64)e) end = off[++rr + 1];    // e < T_all = off[n]: stops at the owning row, empty rows skipped
             tags[q] = (TagT)(stripe_col(rr, swz) | (head ? StripeTag<TagT>::HEAD : 0u));
+            // the same hash behind q: q + 1 is no head (runs that mix hashes: stripe_fix_kernel rewrites their bits)
+            const bool sc = succ && q + 1 < T && key32s[q + 1] == k[u] && (pays[q + 1] >> 32) == (p[u] >> 32);
+            scm |= (u32)sc << u;
             if (bucket) rk[u] = atomicAdd(&s_cnt[e >> lg], 1u);
-            else pos[e] = (u32)q;                         // one window: all of pos[] stays in L2
+            else {
+                pos[e] = (u32)q;                          // one window: all of pos[] (and succ) stays in L2
+                if (sc) atomicOr(succ + (e >> 5), 1u << (e & 31u));
+            }
             // a run that mixes hashes (null worklist: the keys hold every bit, no such runs)
             if (worklist && q && k[u] == kp[u] && p[u] < pp[u]) stripe_note_descent(key32s, pays, q, k[u], worklist, d_count);
         }
@@ -233,7 +249,7 @@ __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__
             const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
             if (q >= T) continue;
             const u32 e = (u32)p[u];
-            bucket[s_base[e >> lg] + rk[u]] = ((u64)e << 32) | q;
+            bucket[s_base[e >> lg] + rk[u]] = succ ? ((u64)((scm >> u) & 1u) << 63) | ((e & wmask) << 32) | q : ((u64)e << 32) | q;
         }
     }
     // STRIPE_TAG_PAD head flags behind the end: the count kernel reads ahead of a group without bounds checks
@@ -241,7 +257,8 @@ __global__ void __launch_bounds__(256) stripe_tag_kernel(const u32* __restrict__
     if (gt < (u64)STRIPE_TAG_PAD) tags[T + gt] = (TagT)StripeTag<TagT>::HEAD;
 }
 
-// the buckets in window order -> pos[e] = q.  Each block takes STRIPE_POS_PER_BLOCK consecutive pairs and blocks
+// the buckets in window order -> pos[e] = q, for buckets of (e << 32 | q) pairs (a tag kernel without `succ`; the
+// product writes pos[] and the successor bits with stripe_pos_sub_kernel below).  Each block takes STRIPE_POS_PER_BLOCK consecutive pairs and blocks
 // start in index order, so the resident blocks work on one or two windows of pos[] at a time; the pairs are read once
 // (evict-first: they must not push the window out of the L2).
 static constexpr int STRIPE_POS_UNROLL = 4;
@@ -258,11 +275,146 @@ __global__ void __launch_bounds__(256) stripe_pos_window_kernel(const u64* __res
         if (v[u] != ~0ull) pos[v[u] >> 32] = (u32)v[u];
 }
 
+// ---- pos[] and succ from shared memory, sub-window by sub-window --------------------------------------------
+// stripe_pos_window_kernel writes each element's position with one scattered 4-byte store into the L2-resident window,
+// and the rate of those L2 writes bounds it.  With succ (see stripe_tag_kernel) the positions take two passes instead:
+// stripe_sub_partition_kernel splits each window's bucket into the buckets of its sub-windows of 2^slg elements
+// (entries move in runs of a tile's entries per sub-window), and stripe_pos_sub_kernel gives one CTA to each
+// sub-window: it scatters the sub-window's positions and successor bits into shared memory and writes its slices of
+// pos[] and succ in whole lines.  As with the windows, every element occurs once, so stripe_window_offsets_kernel at
+// slg gives the sub-buckets' offsets.  Elements of the slices that are not in the stream (a key-range shard's other
+// elements) get position 0xffffffff and bit 0.
+static constexpr int STRIPE_SUB_LOG2 = 14;            // sub-window: 64 KB of positions + 2 KB of bits, three CTAs per SM
+static constexpr int STRIPE_SUB_FANOUT_LOG2 = 11;     // at most 2^11 sub-windows per window (shared counters of the partition)
+static constexpr int STRIPE_SUB_THREADS = 512;
+static constexpr int STRIPE_SUB_U = 12;               // bucket entries per thread and tile of the partition (tiles of 6144)
+static constexpr int STRIPE_SUB_TILE = STRIPE_SUB_U * STRIPE_SUB_THREADS;
+
+// the two levels: window lg (stripe_pos_window_log2, kept within [5, STRIPE_SUB_LOG2 + STRIPE_SUB_FANOUT_LOG2]) and
+// sub-window slg <= lg, 2^slg = STRIPE_SUB_LOG2 or `requested` (elements, rounded down to a power of two), at least
+// 32 elements (whole succ words) and at most 2^STRIPE_SUB_FANOUT_LOG2 per window
+__host__ __device__ __forceinline__ void stripe_pos_levels(u64 l2_bytes, u64 requested, u64 requested_sub, u64 T_all, int& lg, int& slg) {
+    lg = stripe_pos_window_log2(l2_bytes, requested, T_all);
+    if (lg < 5) lg = 5;
+    if (lg > STRIPE_SUB_LOG2 + STRIPE_SUB_FANOUT_LOG2) lg = STRIPE_SUB_LOG2 + STRIPE_SUB_FANOUT_LOG2;
+    slg = STRIPE_SUB_LOG2;
+    if (requested_sub) { slg = 0; while ((2ull << slg) <= requested_sub) ++slg; }
+    if (slg > STRIPE_SUB_LOG2) slg = STRIPE_SUB_LOG2;
+    if (slg < 5) slg = 5;
+    if (slg > lg) slg = lg;
+    if (lg - slg > STRIPE_SUB_FANOUT_LOG2) slg = lg - STRIPE_SUB_FANOUT_LOG2;
+}
+
+// window w = blockIdx.y: its bucket [boff[w], boff[w + 1]) -> the buckets of its 2^(lg - slg) sub-windows (cursors
+// scur, sub-window w << (lg - slg) first), in tiles of STRIPE_SUB_TILE entries.  Each entry takes a rank in its
+// sub-window from a shared counter; the tile is then ordered by sub-window in shared memory (STRIPE_SUB_TILE x 8 B of
+// dynamic shared memory) and written out in that order, so that consecutive lanes store consecutive slots of a
+// sub-bucket: runs of a tile's entries per sub-window (~190 B) instead of one scattered 8-byte store per entry, whose
+// rate of L2 writes would bound the pass as it bounds stripe_pos_window_kernel.
+__global__ void __launch_bounds__(STRIPE_SUB_THREADS, 2) stripe_sub_partition_kernel(const u64* __restrict__ bucket, const u32* __restrict__ boff,
+                                                                                     int lg, int slg, u32* __restrict__ scur,
+                                                                                     u64* __restrict__ sub) {
+    constexpr int U = STRIPE_SUB_U;
+    SMB_DYN_SHARED(u64, s_tile);                          // [STRIPE_SUB_TILE]: the tile, ordered by sub-window
+    SMB_SHARED u32 s_cnt[1 << STRIPE_SUB_FANOUT_LOG2];    // entries of the tile per sub-window, ...
+    SMB_SHARED u32 s_loc[1 << STRIPE_SUB_FANOUT_LOG2];    // ... where its entries start in s_tile, ...
+    SMB_SHARED u32 s_base[1 << STRIPE_SUB_FANOUT_LOG2];   // ... and where the tile's run of its sub-bucket starts
+    const u32 w = blockIdx.y;
+    const u32 ns = 1u << (lg - slg);
+    const u64 b1 = boff[w + 1];
+    const u64 tile = (u64)U * blockDim.x;
+    u32* __restrict__ cur = scur + ((u64)w << (lg - slg));
+    const u32 lane = lane_id();
+    for (u64 t0 = boff[w] + (u64)blockIdx.x * tile; t0 < b1; t0 += (u64)gridDim.x * tile) {
+        for (u32 j = threadIdx.x; j < ns; j += blockDim.x) s_cnt[j] = 0;
+        __syncthreads();
+        u64 v[U];
+        u32 rk[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const u64 i = t0 + (u64)u * blockDim.x + threadIdx.x;
+            v[u] = i < b1 ? ld_stream_u64(bucket + i) : 0ull;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            if (t0 + (u64)u * blockDim.x + threadIdx.x < b1) rk[u] = atomicAdd(&s_cnt[((u32)(v[u] >> 32) & 0x7fffffffu) >> slg], 1u);
+        __syncthreads();
+        if (threadIdx.x < 32) {                           // one warp: exclusive scan of the counts, and the runs' reservations
+            u32 carry = 0;
+            for (u32 j0 = 0; j0 < ns; j0 += 32) {
+                const u32 j = j0 + lane;
+                const u32 c = j < ns ? s_cnt[j] : 0u;
+                u32 x = c;                                // inclusive scan over the warp
+                for (int d = 1; d < 32; d <<= 1) {
+                    const u32 y = __shfl_sync(0xffffffffu, x, (int)lane - d < 0 ? 0 : (int)lane - d);
+                    if ((int)lane >= d) x += y;
+                }
+                if (j < ns) {
+                    s_loc[j] = carry + x - c;
+                    if (c) s_base[j] = atomicAdd(cur + j, c);
+                }
+                carry += __shfl_sync(0xffffffffu, x, 31);
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            if (t0 + (u64)u * blockDim.x + threadIdx.x < b1) s_tile[s_loc[((u32)(v[u] >> 32) & 0x7fffffffu) >> slg] + rk[u]] = v[u];
+        __syncthreads();
+        const u32 len = (u32)min(tile, b1 - t0);
+        for (u32 i = threadIdx.x; i < len; i += blockDim.x) {
+            const u64 x = s_tile[i];
+            const u32 j = ((u32)(x >> 32) & 0x7fffffffu) >> slg;
+            sub[s_base[j] + (i - s_loc[j])] = x;
+        }
+        __syncthreads();                                  // the shared arrays are reused by the next tile
+    }
+}
+
+// sub-window s = blockIdx.x (elements [s << slg, min(T_all, (s + 1) << slg))): its bucket [sboff[s], sboff[s + 1]) ->
+// pos[] and succ through 4 x 2^slg + 2^slg / 8 bytes of dynamic shared memory
+static constexpr int STRIPE_SUB_UNROLL = 4;
+__global__ void __launch_bounds__(STRIPE_SUB_THREADS) stripe_pos_sub_kernel(const u64* __restrict__ sub, const u32* __restrict__ sboff,
+                                                                            u64 T_all, int slg, u32* __restrict__ pos,
+                                                                            u32* __restrict__ succ) {
+    SMB_DYN_SHARED(u32, sub_smem);
+    u32* s_pos = sub_smem;                                // [2^slg]
+    u32* s_succ = sub_smem + (1u << slg);                 // [2^slg / 32]
+    const u64 base = (u64)blockIdx.x << slg;
+    const u32 len = (u32)min((u64)1 << slg, T_all - base);
+    const u32 words = (len + 31) >> 5;
+    const u32 mask = (1u << slg) - 1u;
+    for (u32 i = threadIdx.x; i < len; i += blockDim.x) s_pos[i] = 0xffffffffu;
+    for (u32 i = threadIdx.x; i < words; i += blockDim.x) s_succ[i] = 0;
+    __syncthreads();
+    const u64 b1 = sboff[blockIdx.x + 1];
+    for (u64 i0 = sboff[blockIdx.x] + threadIdx.x; i0 < b1; i0 += (u64)STRIPE_SUB_UNROLL * blockDim.x) {
+        u64 v[STRIPE_SUB_UNROLL];
+#pragma unroll
+        for (int u = 0; u < STRIPE_SUB_UNROLL; ++u) {
+            const u64 i = i0 + (u64)u * blockDim.x;
+            v[u] = i < b1 ? ld_stream_u64(sub + i) : ~0ull;
+        }
+#pragma unroll
+        for (int u = 0; u < STRIPE_SUB_UNROLL; ++u) {
+            if (v[u] == ~0ull) continue;                  // (q < 2^32 - 1: never a real entry)
+            const u32 l = (u32)(v[u] >> 32) & mask;
+            s_pos[l] = (u32)v[u];
+            if (v[u] >> 63) atomicOr(s_succ + (l >> 5), 1u << (l & 31u));
+        }
+    }
+    __syncthreads();
+    u32* __restrict__ dst = pos + base;                   // 2^slg-aligned: whole lines
+    for (u32 i = threadIdx.x; i < len; i += blockDim.x) dst[i] = s_pos[i];
+    for (u32 i = threadIdx.x; i < words; i += blockDim.x) succ[(base >> 5) + i] = s_succ[i];
+}
+
 // the listed runs again, in order (see stripe_note_descent)
 template <typename TagT>
 __global__ void __launch_bounds__(128) stripe_fix_kernel(const u32* __restrict__ key32s, const u64* __restrict__ pays, u64 T,
                                                         const u32* __restrict__ worklist, const u32* __restrict__ d_count,
-                                                        const u64* __restrict__ off, int n, u64* tmp, TagT* tags, u32* pos, u32 swz) {
+                                                        const u64* __restrict__ off, int n, u64* tmp, TagT* tags, u32* pos, u32 swz,
+                                                        u32* succ = nullptr) {
     const u32 count = *d_count;
     const u32 lane = lane_id();
     const u32 warps = gridDim.x * (blockDim.x >> 5);
@@ -290,6 +442,11 @@ __global__ void __launch_bounds__(128) stripe_fix_kernel(const u32* __restrict__
             const u32 e = (u32)v;
             tags[q] = (TagT)(stripe_col(stripe_row_of(off, n, (u64)e), swz) | (first ? StripeTag<TagT>::HEAD : 0u));
             pos[e] = (u32)q;
+            if (succ) {                                   // the run's successor bits; words are shared with other runs' elements,
+                const bool same = q + 1 < tail && (tmp[q + 1] >> 32) == (v >> 32);      // so the bit is flipped by an add:
+                const u32 bit = 1u << (e & 31u);                                            // only this lane changes it
+                if (((succ[e >> 5] & bit) != 0) != same) atomicAdd(succ + (e >> 5), same ? bit : 0u - bit);
+            }
         }
         __syncwarp();
     }
@@ -388,6 +545,8 @@ struct StripeArgs {
     u32 swz;                 // the tags hold stripe_col(row, swz)
     const u32* rows;         // the rows of [row_begin, row_end) in slot order: CTA b counts rows[b * rows_per_block + i]
                              //   (null: index order, slot i counts row row_begin + i)
+    const u32* succ;         // successor bits of the CSR elements (stripe_tag_kernel); null: the tag behind each element
+                             //   is read instead
 };
 
 __host__ __device__ __forceinline__ u32 stripe_slot_row(const StripeArgs& a, int slot) {
@@ -468,9 +627,14 @@ __global__ void __launch_bounds__(1024, CTAS) join_stripe_kernel(StripeArgs a) {
         // a read of 32 tags is only issued when the previous one ended inside the group, whose end is at most T.
         const StripeRowRef row_ref = stripe_row_ref(row_ptr);
         const u32 lane1 = lane + 1u;
-        u32 nxt = HEAD;
-        if (have) nxt = (u32)tags[(size_t)my_q + 1];
-        u32 todo = __ballot_sync(0xffffffffu, nxt < HEAD);
+        u32 todo;
+        if (a.succ) {                                      // one or two words of bits per chunk, not a tag read per element
+            todo = __ballot_sync(0xffffffffu, have && ((a.succ[e >> 5] >> (e & 31u)) & 1u));
+        } else {
+            u32 nxt = HEAD;
+            if (have) nxt = (u32)tags[(size_t)my_q + 1];
+            todo = __ballot_sync(0xffffffffu, nxt < HEAD);
+        }
         while (todo) {
             const int j0 = __ffs(todo) - 1;
             todo &= todo - 1;
