@@ -659,8 +659,12 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     }
     if (T == 0) {                                                   // no hash in this key range: every partial count is zero
         cudaMemsetAsync(js->succ, 0, succ_words * sizeof(u32), s);
-        if (js->tag16) stripe_tag_kernel<u16><<<1, 256, 0, s>>>(nullptr, nullptr, off, nullptr, 0, (u16*)js->tags, js->pos, nullptr, nullptr, 0u);
-        else stripe_tag_kernel<u32><<<1, 256, 0, s>>>(nullptr, nullptr, off, nullptr, 0, (u32*)js->tags, js->pos, nullptr, nullptr, 0u);
+        if (js->tag16)
+            stripe_hash_tag_kernel<u16><<<1, 256, 0, s>>>(nullptr, nullptr, 0, off, nullptr, 0, (u16*)js->tags, js->pos, nullptr, nullptr, 0u,
+                                                          nullptr, nullptr, 0, 0u, nullptr);
+        else
+            stripe_hash_tag_kernel<u32><<<1, 256, 0, s>>>(nullptr, nullptr, 0, off, nullptr, 0, (u32*)js->tags, js->pos, nullptr, nullptr, 0u,
+                                                          nullptr, nullptr, 0, 0u, nullptr);
         count_launches(1);
         if ((e = stripe_make_order(js, scratch, s)) != cudaSuccess) return e;
         *out = guard.release();
@@ -674,48 +678,58 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     stripe_pos_levels(SMB_L2_BYTES, pw ? strtoull(pw, nullptr, 10) : 0ull, psw ? strtoull(psw, nullptr, 10) : 0ull, T_all, pos_lg, sub_lg);
     const u32 nw = (u32)(((T_all - 1) >> pos_lg) + 1);
     const u32 nsub = (u32)(((T_all - 1) >> sub_lg) + 1);
-    u32 *key_a = nullptr, *key_b = nullptr, *eblk = nullptr, *d_count = nullptr, *boff = nullptr, *sboff = nullptr;
-    u64 *pay_a = nullptr, *pay_b = nullptr;
-    if ((e = scratch.alloc((void**)&key_a, Tp * 2 * sizeof(u32))) != cudaSuccess) return e;
-    if ((e = scratch.alloc((void**)&pay_a, Tp * 2 * sizeof(u64))) != cudaSuccess) return e;
-    key_b = key_a + Tp; pay_b = pay_a + Tp;
+    // the sort's bit window: the top 32 significant bits of the hashes, relative to the shard's lo
+    u64 lo = 0, max_rel = max_key;
+    if (js->sharded) {
+        u64 hi;
+        bool bounded;
+        join_shard_range(max_key, shard, n_shards, lo, hi, bounded);
+        max_rel = bounded ? hi - lo - 1 : max_key - lo;
+    }
+    int begin_bit = 0, end_bit = 0;
+    stripe_sort_window(max_rel, begin_bit, end_bit);
+    u64 *hs_in = nullptr, *hs = nullptr, *bucket = nullptr;
+    u32 *es_in = nullptr, *es = nullptr, *eblk = nullptr, *d_count = nullptr, *boff = nullptr, *sboff = nullptr;
+    if ((e = scratch.alloc((void**)&hs, Tp * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&es_in, Tp * 2 * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&bucket, Tp * sizeof(u64))) != cudaSuccess) return e;
+    es = es_in + Tp;
     const u64 nblk = (T_all >> STRIPE_EBLK_LOG2) + 1;
     if ((e = scratch.alloc((void**)&eblk, (nblk + 1) * sizeof(u32))) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&d_count, 16)) != cudaSuccess) return e;
     if ((e = scratch.alloc((void**)&boff, (2 * (size_t)nw + 1) * sizeof(u32))) != cudaSuccess) return e;   // offsets | cursors
     if ((e = scratch.alloc((void**)&sboff, (2 * (size_t)nsub + 1) * sizeof(u32))) != cudaSuccess) return e;  // ... of the sub-windows
     const unsigned grid = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_SMS * 32);
-    const int low_bits = stripe_low_bits(max_key);
-    // 1. 32-bit sort keys (top bits of the hashes) + payloads (low bits, element index)
+    // 1. the sort's input: the resident hashes themselves and an iota of their elements, or a shard's slices gathered
+    //    as (hash - lo, element)
     if (js->sharded) {
+        if ((e = scratch.alloc((void**)&hs_in, Tp * sizeof(u64))) != cudaSuccess) return e;
         const int blocks = n < SMB_SMS * 16 ? n : SMB_SMS * 16;
-        stripe_keys_slice_kernel<<<blocks, 256, 0, s>>>(h, js->ebeg, d_doff, n, low_bits, key_a, pay_a);
+        stripe_gather_slice_kernel<<<blocks, 256, 0, s>>>(h, js->ebeg, d_doff, n, lo, hs_in, es_in);
     } else {
-        stripe_keys_kernel<<<grid, 256, 0, s>>>(h, T, low_bits, key_a, pay_a);
+        stripe_iota_kernel<<<grid, 256, 0, s>>>(T, es_in);
     }
     count_launches(1);
-    // 2. four radix passes (fewer when the keys are short)
-    int key_bits = key_bit_length(max_key);
-    if (key_bits > 32) key_bits = 32;
+    // 2. four radix passes over the window (fewer when the hashes are short)
+    const u64* keys_in = js->sharded ? hs_in : h;
     size_t sort_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, key_a, key_b, pay_a, pay_b, (long long)T, 0, key_bits, s);
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys_in, hs, es_in, es, (long long)T, begin_bit, end_bit, s);
     void* d_sort = nullptr;
     if ((e = scratch.alloc(&d_sort, sort_bytes)) != cudaSuccess) return e;
-    cub::DeviceRadixSort::SortPairs(d_sort, sort_bytes, key_a, key_b, pay_a, pay_b, (long long)T, 0, key_bits, s);
+    cub::DeviceRadixSort::SortPairs(d_sort, sort_bytes, keys_in, hs, es_in, es, (long long)T, begin_bit, end_bit, s);
     count_launches(1);
     // 3. tags + inverse permutation + successor bits: the tag kernel appends (element, position, bit) entries to the
-    //    buckets of the pos[] windows (pay_a is free: 8 B per element), the partition splits them into the buckets of
-    //    the sub-windows (the sort's temporary storage is free: it holds the keys' and payloads' second buffers), and
-    //    the sub-window pass writes pos[] and succ from shared memory; when pos[] is one window it stays in L2 as a whole
-    //    and the tag kernel stores positions and bits directly.  Runs of equal keys that hold more than one hash are
-    //    noticed on the way (key_a is free: worklist) and redone in order after the position pass, one warp per run
-    //    (pay_a is free again: the ordered payloads of those runs)
-    u32* worklist = low_bits ? key_a : nullptr;
-    if (low_bits) cudaMemsetAsync(d_count, 0, sizeof(u32), s);
+    //    buckets of the pos[] windows, the partition splits them into the buckets of the sub-windows (the sort's
+    //    temporary storage is free: it holds cub's alternate buffers), and the sub-window pass writes pos[] and succ
+    //    from shared memory; when pos[] is one window it stays in L2 as a whole and the tag kernel stores positions and
+    //    bits directly.  Runs of equal window bits that hold more than one hash are noticed on the way (the iota is
+    //    free: worklist) and redone in order after the position pass, one warp per run (the buckets are free again:
+    //    the ordered positions of those runs)
+    u32* worklist = begin_bit ? es_in : nullptr;
+    if (begin_bit) cudaMemsetAsync(d_count, 0, sizeof(u32), s);
     stripe_eblk_kernel<<<(unsigned)std::min<u64>((nblk + 255) / 256, (u64)SMB_SMS * 8), 256, 0, s>>>(off, n, T_all, eblk);
     count_launches(1);
     const bool windows = nw > 1;
-    u64* bucket = windows ? pay_a : nullptr;
     const u64* doff = js->sharded ? d_doff : off;
     if (windows) {
         stripe_window_offsets_kernel<<<(nw + 256) / 256, 256, 0, s>>>(off, n, js->ebeg, js->eend, doff, T_all, T, pos_lg, nw, boff, boff + nw + 1);
@@ -727,11 +741,11 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
     }
     const unsigned tag_grid = (unsigned)std::min<u64>((T + STRIPE_TAG_TILE - 1) / STRIPE_TAG_TILE, (u64)SMB_SMS * 16);
     if (js->tag16)
-        stripe_tag_kernel<u16><<<tag_grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u16*)js->tags, js->pos, worklist, d_count, js->swz,
-                                                        bucket, boff + nw + 1, pos_lg, nw, js->succ);
+        stripe_hash_tag_kernel<u16><<<tag_grid, 256, 0, s>>>(hs, es, begin_bit, off, eblk, T, (u16*)js->tags, js->pos, worklist, d_count, js->swz,
+                                                             windows ? bucket : nullptr, boff + nw + 1, pos_lg, nw, js->succ);
     else
-        stripe_tag_kernel<u32><<<tag_grid, 256, 0, s>>>(key_b, pay_b, off, eblk, T, (u32*)js->tags, js->pos, worklist, d_count, js->swz,
-                                                        bucket, boff + nw + 1, pos_lg, nw, js->succ);
+        stripe_hash_tag_kernel<u32><<<tag_grid, 256, 0, s>>>(hs, es, begin_bit, off, eblk, T, (u32*)js->tags, js->pos, worklist, d_count, js->swz,
+                                                             windows ? bucket : nullptr, boff + nw + 1, pos_lg, nw, js->succ);
     count_launches(1);
     if (windows) {
         u64* sub = (u64*)d_sort;
@@ -740,7 +754,7 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
         const size_t part_smem = (size_t)STRIPE_SUB_TILE * sizeof(u64);
         if ((e = cudaFuncSetAttribute(stripe_sub_partition_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)part_smem)) != cudaSuccess)
             return e;
-        stripe_sub_partition_kernel<<<dim3((unsigned)chunks, nw), STRIPE_SUB_THREADS, part_smem, s>>>(pay_a, boff, pos_lg, sub_lg, sboff + nsub + 1,
+        stripe_sub_partition_kernel<<<dim3((unsigned)chunks, nw), STRIPE_SUB_THREADS, part_smem, s>>>(bucket, boff, pos_lg, sub_lg, sboff + nsub + 1,
                                                                                                        sub);
         const size_t sub_smem = ((size_t)4 << sub_lg) + ((size_t)1 << sub_lg) / 8;
         if ((e = cudaFuncSetAttribute(stripe_pos_sub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sub_smem)) != cudaSuccess) return e;
@@ -750,13 +764,14 @@ cudaError_t join_stripe_create_shard(const u64* h, const u64* off, int n, u64 T_
         stripe_pos_sub_kernel<<<nsub, STRIPE_SUB_THREADS, sub_smem, s>>>(sub, sboff, T_all, sub_lg, js->pos, js->succ);
         count_launches(2);
     }
-    if (low_bits) {
+    if (begin_bit) {
+        u32* tmp = (u32*)bucket;
         if (js->tag16)
-            stripe_fix_kernel<u16><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u16*)js->tags, js->pos, js->swz,
-                                                               js->succ);
+            stripe_hash_fix_kernel<u16><<<SMB_SMS * 4, 128, 0, s>>>(hs, es, begin_bit, T, worklist, d_count, off, n, tmp, (u16*)js->tags, js->pos,
+                                                                    js->swz, js->succ);
         else
-            stripe_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(key_b, pay_b, T, worklist, d_count, off, n, pay_a, (u32*)js->tags, js->pos, js->swz,
-                                                               js->succ);
+            stripe_hash_fix_kernel<u32><<<SMB_SMS * 4, 128, 0, s>>>(hs, es, begin_bit, T, worklist, d_count, off, n, tmp, (u32*)js->tags, js->pos,
+                                                                    js->swz, js->succ);
         count_launches(1);
     }
     if ((e = stripe_make_order(js, scratch, s)) != cudaSuccess) return e;

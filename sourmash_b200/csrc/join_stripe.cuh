@@ -17,13 +17,14 @@
 //   tags[q] = row of sorted element q, top bit set on the first element of a group   (u16 if n < 32768: the
 //             whole stream of a 10 000 x 5 000 set is then 100 MB instead of 200 MB; each CTA reads it front to back)
 //   pos[e]  = sorted position of CSR element e
-// and is built with FOUR radix passes instead of seven: the sort key is the top 32 significant bits of the
-// hash, the remaining low bits travel in the 64-bit payload in front of the element index
-// (payload = low bits << 32 | e).  Elements with equal 32-bit keys form a run, kept in CSR order by the
-// stable sort; nearly every run is one group.  The rare runs that mix different hashes (expected
-// distinct^2 / 2^33) are recognised by a payload that is smaller than its predecessor's and redone in order
-// by one warp each -- ascending payloads = ascending (low bits, element) = groups contiguous, rows ascending.
-// Because the key is a prefix of the hash, the stream is in hash order and every row walks it front to back.
+// and is built with FOUR radix passes instead of seven: the hashes are sorted on their top 32 significant bits.
+// Elements with equal top bits form a run, kept in CSR order by the stable sort; nearly every run is one group.
+// The rare runs that mix different hashes (expected distinct^2 / 2^33) are recognised by a hash (or payload)
+// smaller than its predecessor's and redone in (hash, element) order by one warp each -- groups contiguous, rows
+// ascending.  Because the key is a prefix of the hash, the stream is in hash order and every row walks it front
+// to back.  The product sorts the resident hashes themselves (stripe_hash_tag_kernel below); stripe_keys_kernel,
+// stripe_tag_kernel and stripe_fix_kernel, which sort a copy as 32-bit keys + payloads (low bits << 32 | e), are
+// kept for the emulator drivers under tests/host_emul that run them.
 #pragma once
 #include "common.cuh"
 
@@ -447,6 +448,177 @@ __global__ void __launch_bounds__(128) stripe_fix_kernel(const u32* __restrict__
                 const u32 bit = 1u << (e & 31u);                                            // only this lane changes it
                 if (((succ[e >> 5] & bit) != 0) != same) atomicAdd(succ + (e >> 5), same ? bit : 0u - bit);
             }
+        }
+        __syncwarp();
+    }
+}
+
+// ---- stream construction from the hashes themselves ---------------------------------------------------------
+// The product sorts the resident u64 hashes directly (cub keys = the hashes, values = the element indices) on the
+// bit window [end - 32, end) of their `end` significant bits, instead of first writing a copy of every hash as a 32-bit
+// key + 64-bit payload (400 MB read, 600 MB written on 5e7 elements): an iota of the indices (200 MB) replaces that
+// copy, every radix pass still moves 12 B per element, and the sorted stream carries the full hash, so head and
+// successor tests compare two hashes.  Elements with equal window bits form a run, in element order (stable sort,
+// input in CSR order); a run holds more than one hash exactly when its hashes descend somewhere, and those runs are
+// listed by stripe_hash_tag_kernel and redone in (hash, element) order by stripe_hash_fix_kernel.  A key-range shard
+// sorts hash - lo, whose order and equalities are the hashes'; its window is the top 32 bits of the range's width.
+
+// the sort's bit window for hashes (relative to the shard's lo) no larger than max_rel
+__host__ __device__ __forceinline__ void stripe_sort_window(u64 max_rel, int& begin_bit, int& end_bit) {
+    end_bit = 1;
+    while (end_bit < 64 && (max_rel >> end_bit)) ++end_bit;
+    begin_bit = end_bit > 32 ? end_bit - 32 : 0;
+}
+
+__global__ void __launch_bounds__(256) stripe_iota_kernel(u64 T, u32* __restrict__ es) {
+    for (u64 e = (u64)blockIdx.x * blockDim.x + threadIdx.x; e < T; e += (u64)gridDim.x * blockDim.x) es[e] = (u32)e;
+}
+
+// a shard's row slices -> (hash - lo, element index in the whole CSR), written back to back
+__global__ void __launch_bounds__(256) stripe_gather_slice_kernel(const u64* __restrict__ h, const u64* __restrict__ ebeg,
+                                                                 const u64* __restrict__ dst_off, int n, u64 lo,
+                                                                 u64* __restrict__ hs, u32* __restrict__ es) {
+    for (int r = blockIdx.x; r < n; r += gridDim.x) {
+        const u64 src = ebeg[r], d0 = dst_off[r], m = dst_off[r + 1] - d0;
+        for (u64 i = threadIdx.x; i < m; i += blockDim.x) {
+            hs[d0 + i] = h[src + i] - lo;
+            es[d0 + i] = (u32)(src + i);
+        }
+    }
+}
+
+// q: a descent (same window bits as q - 1, smaller hash).  The thread that meets the run's FIRST descent appends the
+// run's head to the worklist (it can hold every element, so it never overflows).
+__device__ __forceinline__ void stripe_note_hash_descent(const u64* __restrict__ hs, u64 q, int shift, u32* __restrict__ worklist,
+                                                         u32* __restrict__ d_count) {
+    const u64 k = hs[q] >> shift;
+    u64 p = q - 1;
+    while (p > 0 && (hs[p - 1] >> shift) == k) {
+        if (hs[p] < hs[p - 1]) return;
+        --p;
+    }
+    worklist[atomicAdd(d_count, 1u)] = (u32)p;
+}
+
+// stripe_tag_kernel for the stream of sorted hashes `hs` and their elements `es` (window bits = hs >> shift; null
+// worklist: the window holds every bit, no run mixes hashes): tags, position buckets (or pos[] and succ directly when
+// pos[] is one window), successor bits, and the worklist of runs that mix hashes.
+template <typename TagT>
+__global__ void __launch_bounds__(256) stripe_hash_tag_kernel(const u64* __restrict__ hs, const u32* __restrict__ es, int shift,
+                                                             const u64* __restrict__ off, const u32* __restrict__ eblk, u64 T,
+                                                             TagT* __restrict__ tags, u32* __restrict__ pos, u32* __restrict__ worklist,
+                                                             u32* __restrict__ d_count, u32 swz, u64* __restrict__ bucket,
+                                                             u32* __restrict__ cur, int lg, u32 nw, u32* __restrict__ succ) {
+    constexpr int U = STRIPE_TAG_U;
+    SMB_SHARED u32 s_cnt[STRIPE_MAX_WINDOWS];             // elements of the tile per window, then ...
+    SMB_SHARED u32 s_base[STRIPE_MAX_WINDOWS];            // ... where the tile's run of each bucket starts
+    const u64 tile = (u64)U * blockDim.x;
+    const u64 wmask = (1ull << lg) - 1ull;
+    for (u64 t0 = (u64)blockIdx.x * tile; t0 < T; t0 += (u64)gridDim.x * tile) {
+        if (bucket) {
+            for (u32 w = threadIdx.x; w < nw; w += blockDim.x) s_cnt[w] = 0;
+            __syncthreads();
+        }
+        u64 x[U], xp[U];
+        u32 ev[U], r[U], rk[U];
+        u64 nx[U];
+        u32 scm = 0;                                      // bit u: the successor bit of position u
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
+            const bool in = q < T;
+            x[u] = in ? hs[q] : 0;
+            ev[u] = in ? es[q] : 0;
+            xp[u] = (in && q) ? hs[q - 1] : 0;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) r[u] = eblk[ev[u] >> STRIPE_EBLK_LOG2];
+#pragma unroll
+        for (int u = 0; u < U; ++u) nx[u] = off[r[u] + 1];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
+            if (q >= T) continue;
+            const u32 e = ev[u];
+            const bool head = q == 0 || x[u] != xp[u];
+            u32 rr = r[u];
+            u64 end = nx[u];
+            while (end <= (u64)e) end = off[++rr + 1];    // e < T_all = off[n]: stops at the owning row, empty rows skipped
+            tags[q] = (TagT)(stripe_col(rr, swz) | (head ? StripeTag<TagT>::HEAD : 0u));
+            // the same hash behind q (runs that mix hashes: stripe_hash_fix_kernel rewrites their bits)
+            const bool sc = q + 1 < T && hs[q + 1] == x[u];
+            scm |= (u32)sc << u;
+            if (bucket) rk[u] = atomicAdd(&s_cnt[e >> lg], 1u);
+            else {
+                pos[e] = (u32)q;                          // one window: all of pos[] (and succ) stays in L2
+                if (sc) atomicOr(succ + (e >> 5), 1u << (e & 31u));
+            }
+            if (worklist && q && x[u] < xp[u] && (x[u] >> shift) == (xp[u] >> shift)) stripe_note_hash_descent(hs, q, shift, worklist, d_count);
+        }
+        if (!bucket) continue;                            // uniform: a kernel parameter
+        __syncthreads();
+        for (u32 w = threadIdx.x; w < nw; w += blockDim.x) {
+            const u32 c = s_cnt[w];
+            if (c) s_base[w] = atomicAdd(cur + w, c);
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const u64 q = t0 + (u64)u * blockDim.x + threadIdx.x;
+            if (q >= T) continue;
+            const u32 e = ev[u];
+            bucket[s_base[e >> lg] + rk[u]] = ((u64)((scm >> u) & 1u) << 63) | ((e & wmask) << 32) | q;
+        }
+    }
+    // STRIPE_TAG_PAD head flags behind the end: the count kernel reads ahead of a group without bounds checks
+    const u64 gt = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gt < (u64)STRIPE_TAG_PAD) tags[T + gt] = (TagT)StripeTag<TagT>::HEAD;
+}
+
+// the listed runs again, in (hash, element) order: one warp per run.  Each element is ranked in its run -- rank =
+// #{smaller hashes} + #{equal hashes in front of it}, elements ascend inside a run -- and its stream position is written
+// to `tmp` at the run's head + rank (a free buffer, slots of the run's own positions); then the run's tags, positions and
+// successor bits are derived from that order, after the position pass, whose positions of these runs they overwrite.
+template <typename TagT>
+__global__ void __launch_bounds__(128) stripe_hash_fix_kernel(const u64* __restrict__ hs, const u32* __restrict__ es, int shift, u64 T,
+                                                             const u32* __restrict__ worklist, const u32* __restrict__ d_count,
+                                                             const u64* __restrict__ off, int n, u32* tmp, TagT* tags, u32* pos, u32 swz,
+                                                             u32* succ) {
+    const u32 count = *d_count;
+    const u32 lane = lane_id();
+    const u32 warps = gridDim.x * (blockDim.x >> 5);
+    for (u32 i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < count; i += warps) {
+        const u64 head = worklist[i];
+        const u64 k = hs[head] >> shift;
+        u64 tail = head + 1;                              // end of the run: 32 positions probed at a time
+        for (;;) {
+            const u64 q = tail + lane;
+            const bool same = q < T && (hs[q] >> shift) == k;
+            const u32 m = __ballot_sync(0xffffffffu, !same);
+            if (m) { tail += (u64)(__ffs((int)m) - 1); break; }
+            tail += 32;
+        }
+        for (u64 a = head + lane; a < tail; a += 32) {
+            const u64 v = hs[a];
+            u64 rank = 0;
+            for (u64 b = head; b < tail; ++b) {
+                const u64 w = hs[b];
+                rank += (w < v || (w == v && b < a)) ? 1u : 0u;
+            }
+            tmp[head + rank] = (u32)a;
+        }
+        __syncwarp();                                     // tmp[head, tail) written by this warp, read by it below
+        for (u64 q = head + lane; q < tail; q += 32) {
+            const u64 v = hs[tmp[q]];
+            const u32 e = es[tmp[q]];
+            const bool first = q == head || hs[tmp[q - 1]] != v;
+            tags[q] = (TagT)(stripe_col(stripe_row_of(off, n, (u64)e), swz) | (first ? StripeTag<TagT>::HEAD : 0u));
+            pos[e] = (u32)q;
+            // the run's successor bits; words are shared with other runs' elements, so the bit is flipped by an add:
+            // only this lane changes it
+            const bool same = q + 1 < tail && hs[tmp[q + 1]] == v;
+            const u32 bit = 1u << (e & 31u);
+            if (((succ[e >> 5] & bit) != 0) != same) atomicAdd(succ + (e >> 5), same ? bit : 0u - bit);
         }
         __syncwarp();
     }
