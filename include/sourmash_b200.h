@@ -342,6 +342,14 @@ void smb_one_vs_many(const uint64_t *query, uintptr_t n_query, const SmbSketchSe
 /* the same with the (sorted) query and the n_rows counters in device memory: nothing crosses PCIe */
 void smb_one_vs_many_dev(const uint64_t *d_query, uintptr_t n_query, const SmbSketchSet *db,
                          uint32_t *d_common_out);
+/* Which query hashes the listed rows hold: covered_out[p] = 1 iff query[p] is in some row rows[i], else 0 (n_query
+ * bytes).  The query is sorted, unique and at the set's scaled, as for smb_one_vs_many; rows may repeat.  The rows are
+ * probed in place in the resident set -- one probe of the query's directory per element of the listed rows -- which is
+ * what prefetch's matched / unmatched query hashes (commands.py: prefetch, --save-matching-hashes /
+ * --save-unmatched-hashes) need without merging the whole query once per match.  A row index >= n_rows is an error,
+ * raised before anything is launched; an empty query or row list gives zeros without a launch. */
+void smb_query_covered(const uint64_t *query, uintptr_t n_query, const SmbSketchSet *db, const uint32_t *rows,
+                       uintptr_t n_rows, uint8_t *covered_out);
 /* Index.search_abund (src/sourmash/index/__init__.py:172-200): the angular similarity (KmerMinHash::angular_similarity,
  * sketch/minhash.rs:635-680) of one abundance query (sorted-unique hashes q, abundances q_abunds) with every row of a
  * set that carries abundances, over the hashes <= max_hash of both sides (UINT64_MAX: all of them) -- what

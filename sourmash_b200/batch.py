@@ -314,6 +314,21 @@ def one_vs_many_device(d_query_ptr, n_query, db, d_counts_ptr):
              ffi.cast("uint32_t *", int(d_counts_ptr)))
 
 
+def query_covered(query, db, rows):
+    """Boolean mask over ``query`` (sorted-unique u64, at the set's scaled): True where some row ``rows[i]`` of ``db``
+    holds the hash.  ``query[mask]`` is the union of the rows' intersections with the query (prefetch's matched hashes),
+    ``query[~mask]`` the rest.  The rows are probed in place on the device; a row may be listed twice."""
+    q = _u64(query)
+    r = np.asarray(rows, dtype=np.int64).ravel()
+    if len(r) and (r.min() < 0 or r.max() > 0xFFFFFFFF):              # would wrap as uint32; the library checks the rest
+        raise ValueError(f"row index {int(r[(r < 0) | (r > 0xFFFFFFFF)][0])} out of range for a set of {len(db)} rows")
+    r = np.ascontiguousarray(r, dtype=np.uint32)
+    out = np.zeros(len(q), dtype=np.uint8)
+    rustcall(lib.smb_query_covered, _ptr(q, "uint64_t *"), len(q), db._ptr, _ptr(r, "uint32_t *"), len(r),
+             _ptr(out, "uint8_t *"))
+    return out.view(np.bool_)
+
+
 def search_angular(q_hashes, q_abunds, sset, max_hash):
     """Angular similarity of one abundance query (sorted-unique ``q_hashes``, ``q_abunds``) with every row of ``sset``
     (which must carry abundances), over the hashes <= ``max_hash`` of both sides: a float64 ``(len(sset),)`` array,

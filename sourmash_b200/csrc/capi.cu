@@ -2313,6 +2313,34 @@ void smb_one_vs_many(const uint64_t* query, uintptr_t n_query, const SmbSketchSe
     });
 }
 
+// prefetch's matched / unmatched query hashes (commands.py: prefetch, ident_mh / noident_mh) as one device pass over the
+// passing rows instead of a merge of the whole query per match
+void smb_query_covered(const uint64_t* query, uintptr_t n_query, const SmbSketchSet* db, const uint32_t* rows,
+                       uintptr_t n_rows, uint8_t* covered_out) {
+    guarded_void([&] {
+        for (uintptr_t i = 0; i < n_rows; ++i)
+            if (rows[i] >= db->n_rows)
+                fail(SOURMASH_ERROR_CODE_MSG, "row index " + std::to_string(rows[i]) + " out of range for a set of " +
+                                                  std::to_string(db->n_rows) + " rows");
+        for (uintptr_t i = 1; i < n_query; ++i)
+            if (query[i] <= query[i - 1]) fail(SOURMASH_ERROR_CODE_MSG, "query hashes are not sorted and unique");
+        std::fill(covered_out, covered_out + n_query, (uint8_t)0);
+        if (n_query == 0 || n_rows == 0) return;
+        cudaStream_t s = need_gpu();
+        DevBuf<uint64_t> d_q(n_query, s);
+        DevBuf<uint32_t> d_rows(n_rows, s);
+        DevBuf<uint8_t> d_cov(n_query, s);
+        d_q.upload(query, n_query);
+        d_rows.upload(rows, n_rows);
+        if (t_profiling) t_timer_hash.begin(s);
+        CK(smb::launch_query_cover(d_q.p, n_query, query[n_query - 1], db->d_hashes, db->d_off, d_rows.p, n_rows,
+                                   d_cov.p, s));
+        if (t_profiling) t_timer_hash.end(s);
+        d_cov.download(covered_out, n_query);
+        sync(s);
+    });
+}
+
 void smb_one_vs_many_dev(const uint64_t* d_query, uintptr_t n_query, const SmbSketchSet* db, uint32_t* d_common_out) {
     guarded_void([&] {
         cudaStream_t s = need_gpu();

@@ -1053,6 +1053,37 @@ cudaError_t angular_search(AngularSearchArgs a, cudaStream_t s) {
     return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------
+// Which query keys the listed rows hold (query_cover_kernel): the global directory and bitmap of the one-vs-many path,
+// sized as one_vs_many_dev sizes them, then one warp per listed row.  covered (nq bytes) is zeroed here.
+// ------------------------------------------------------------------------------------
+cudaError_t launch_query_cover(const u64* q, u64 nq, u64 q_max, const u64* hB, const u64* offB, const u32* rows,
+                               u64 n_rows, u8* covered, cudaStream_t s) {
+    cudaError_t e;
+    if (nq == 0) return cudaSuccess;
+    if ((e = cudaMemsetAsync(covered, 0, nq, s)) != cudaSuccess) return e;
+    if (n_rows == 0) return cudaSuccess;
+    int nb_log2 = 12;
+    while (nb_log2 < 26 && (1ull << nb_log2) < 2 * nq) ++nb_log2;
+    int shift = 0;
+    while (shift < 63 && (q_max >> shift) >= (1ull << nb_log2)) ++shift;
+    const u64 nb = (q_max >> shift) + 1;
+    const int fine_log2 = 3;
+    const size_t bm_words = ((size_t)nb << fine_log2) / 32 + 2;
+    JoinScratch scratch(s);
+    u32 *dir = nullptr, *bm = nullptr;
+    if ((e = scratch.alloc((void**)&dir, (nb + 2) * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&bm, bm_words * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(bm, 0, bm_words * sizeof(u32), s)) != cudaSuccess) return e;
+    launch_build_global_dir(q, nq, shift, nb, dir, s);
+    launch_build_query_bitmap(q, nq, shift, fine_log2, bm, s);
+    u64 blocks = (n_rows + 7) / 8;
+    if (blocks > (u64)SMB_SMS * 16) blocks = (u64)SMB_SMS * 16;
+    query_cover_kernel<<<(unsigned)blocks, 256, 0, s>>>(q, nq, dir, (u32)shift, nb, bm, fine_log2, hB, offB, rows,
+                                                        n_rows, covered); count_launches(1);
+    return cudaGetLastError();
+}
+
 void launch_index_count(const DbIndex* ix, const u64* q, u64 nq, u32* counts, cudaStream_t s) {
     if (nq == 0 || ix->view.n_keys == 0) return;
     u64 blocks = (nq + 255) / 256;

@@ -355,6 +355,12 @@ struct AngularSearchArgs {
 };
 cudaError_t angular_search(AngularSearchArgs a, cudaStream_t s);
 
+// covered[p] = 1 iff q[p] (sorted-unique, q_max = q[nq - 1]) is held by one of the rows rows[0..n_rows) of the CSR
+// (hB, offB); the other nq bytes are 0.  Rows are read in place.
+cudaError_t launch_query_cover(const uint64_t* q, uint64_t nq, uint64_t q_max, const uint64_t* hB,
+                               const uint64_t* offB, const uint32_t* rows, uint64_t n_rows, uint8_t* covered,
+                               cudaStream_t s);
+
 // kernel-launch accounting (smb_kernel_launches)
 void count_launches(int n);
 

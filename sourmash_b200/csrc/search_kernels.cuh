@@ -124,6 +124,55 @@ __global__ void __launch_bounds__(256) one_vs_many_global_kernel(
     }
 }
 
+// covered[p] = 1 for every query key q[p] held by one of the listed rows (prefetch's matched / unmatched query hashes).
+// One warp per listed row, read in place from the CSR; every element probes the bitmap and directory exactly as
+// one_vs_many_global_kernel does.  Writers of one byte all store 1, so no atomics; a row listed twice is harmless.
+__global__ void __launch_bounds__(256) query_cover_kernel(
+    const u64* __restrict__ q, u64 nq, const u32* __restrict__ dir, u32 shift, u64 nbk,
+    const u32* __restrict__ bitmap, int fine_log2, const u64* __restrict__ hB,
+    const u64* __restrict__ offB, const u32* __restrict__ rows, u64 n_rows, u8* __restrict__ covered) {
+    const u32 bm_shift = shift >= (u32)fine_log2 ? shift - (u32)fine_log2 : 0u;
+    const int lane = lane_id();
+    const u64 wstride = (u64)gridDim.x * (blockDim.x >> 5);
+    constexpr int U = 4;
+    for (u64 j = (u64)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); j < n_rows; j += wstride) {
+        const u32 r = rows[j];
+        const u64* row = hB + offB[r];
+        const u64 n = offB[r + 1] - offB[r];
+        for (u64 base = 0; base < n; base += 32 * U) {
+            u64 x[U];
+            u32 word[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const u64 e = base + (u64)u * 32 + lane;
+                x[u] = e < n ? ld_nc_u64(row + e) : SMB_U64_MAX;
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                // padding lanes by index, not by value: a query holding UINT64_MAX (scaled = 1) covers the padding key
+                const bool in_range = base + (u64)u * 32 + lane < n && (x[u] >> shift) < nbk;
+                word[u] = 0u;
+                if (in_range) {
+                    const u64 bit = x[u] >> bm_shift;
+                    word[u] = (__ldg(bitmap + (bit >> 5)) >> (bit & 31)) & 1u;
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                if (word[u]) {
+                    const u64 b = x[u] >> shift;
+                    u64 p = dir[b];
+                    const u64 pe = dir[b + 1];
+                    for (; p < pe; ++p) {
+                        const u64 k = ld_nc_u64(q + p);
+                        if (k >= x[u]) { if (k == x[u]) covered[p] = 1; break; }
+                    }
+                }
+            }
+        }
+    }
+}
+
 template <bool KEEP_COMMON>
 __global__ void __launch_bounds__(1024) setop_rows_kernel(const u64* __restrict__ a, u64 na,
                                                          const u64* __restrict__ b, u64 nb,

@@ -209,7 +209,7 @@ def _gather_row(p, r, rank, ab, remaining, left_weight, c0, m, *, estimate_ani_c
 
 def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, estimate_ani_ci=False,
                      names=None, md5s=None, filenames=None, query_name="", query_filename="", max_rounds=None,
-                     noident_hashes=None, locations=None, query_orig=None):
+                     noident_hashes=None, locations=None, query_orig=None, stats=None):
     """Min-set-cover of ``query_mh`` by the rows of the GPU-resident SketchSet ``db`` (same ksize,
     seed and scaled as the query; use ``SketchSet.downsample`` / ``SignatureSet.to_sketchset``).
     Returns the list of GatherRow in pick order -- the reference's GatherDatabases loop with the
@@ -219,11 +219,18 @@ def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, es
     from its prefetch stage, commands.py:894-922,973): they are taken out of the query that is searched,
     but stay in the denominators -- query_bp, query_n_hashes, f_orig_query, f_unique_to_query,
     total_weighted_hashes -- and in remaining_bp (GatherDatabases.__init__ / __next__,
-    search.py:803-818,910-944; GatherResult.build_gather_result, search.py:553-590)."""
+    search.py:803-818,910-944; GatherResult.build_gather_result, search.py:553-590).
+
+    ``stats`` (a dict, optional) receives what the rounds leave behind: ``q_hashes`` (the searched query), ``alive``
+    (the mask of its hashes no pick took), ``counts0`` (every row's overlap with it, the prefetch stage) and
+    ``min_count`` (the least overlap of a row that takes part).  Without a round: ``counts0`` is None."""
     p = _prepare_query(query_mh, threshold_bp=threshold_bp, ignore_abundance=ignore_abundance,
                        noident_hashes=noident_hashes, query_orig=query_orig, query_name=query_name,
                        query_filename=query_filename)
     rows = []
+    if stats is not None:
+        stats.update(q_hashes=p.q_hashes if p is not None else query_mh._mins_array(), counts0=None, min_count=None)
+        stats["alive"] = np.ones(len(stats["q_hashes"]), dtype=bool)
     if p is None or len(db) == 0:
         return rows
     scaled = query_mh.scaled
@@ -231,6 +238,8 @@ def gather_databases(query_mh, db, *, threshold_bp=0, ignore_abundance=False, es
     sizes = db.sizes()
     counts0 = B.one_vs_many(q_hashes, db)                     # |match ∩ original query| for every row
     alive = np.ones(len(q_hashes), dtype=bool)                 # hashes of the searched query not yet covered
+    if stats is not None:
+        stats.update(counts0=counts0, alive=alive, min_count=p.min_count)
     remaining = len(q_hashes)
     rowmap = None
     if p.min_count > 1:                                        # the session's min_count is a hint; the rule is enforced here
@@ -348,10 +357,11 @@ def _min_count_of_given_query(threshold_bp, query_orig, query_len):
 
 
 def prefetch_database(query_mh, db, threshold_bp, *, estimate_ani_ci=False, names=None, md5s=None, filenames=None,
-                      query_name="", query_filename="", query_orig=None, match_orig=None):
+                      query_name="", query_filename="", query_orig=None, match_orig=None, counts=None):
     """All rows of ``db`` sharing at least ``threshold_bp`` with the query, in database order, as
     dictionaries with the reference's prefetch columns (search.py:953-998 + PrefetchResult
-    :357-470).  One pass of the one-vs-many kernel; everything else is per-match scalar work."""
+    :357-470).  One pass of the one-vs-many kernel; everything else is per-match scalar work.  ``counts``: the overlaps
+    of that pass when the caller already has them (gather's prefetch stage), so the pass is not run again."""
     if not query_mh.scaled:
         raise TypeError("query signature must be calculated with scaled")
     scaled, ksize = query_mh.scaled, query_mh.ksize
@@ -363,7 +373,8 @@ def prefetch_database(query_mh, db, threshold_bp, *, estimate_ani_ci=False, name
         calc_threshold_from_bp(threshold_bp, int(query_orig[1]), int(query_orig[0]))
     else:
         calc_threshold_from_bp(threshold_bp, scaled, nq)
-    counts = B.one_vs_many(q, db)
+    if counts is None:
+        counts = B.one_vs_many(q, db)
     sizes = db.sizes()
     cache = {}
     q_ok = _size_ok(nq, scaled, cache)

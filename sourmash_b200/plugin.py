@@ -229,6 +229,7 @@ def _load_query_and_db(args):
     if len(queries) != 1:
         raise ValueError(f"need exactly one query sketch in '{args.query}' (found {len(queries)}); select with -k")
     query = queries[0]
+    given_mh = query.minhash
     if args.scaled and int(args.scaled) > query.minhash.scaled:        # --scaled: the query itself is downsampled first, and that
         with query.update() as query:                                  # sketch is "the query" of the reports (commands.py: gather)
             query.minhash = query.minhash.downsample(scaled=int(args.scaled))
@@ -254,7 +255,63 @@ def _load_query_and_db(args):
     # the sketches as given: the reports quote their sizes and the query's md5, the comparisons run at `scaled`
     meta["query_orig"] = (len(query.minhash), query.minhash.scaled, query.md5sum())
     meta["match_orig"] = (db.n_mins[rows].astype(np.int64), db.python_scaled()[rows].astype(np.int64))
-    return qmh, sset, meta
+    # what the signature outputs need: the database rows as loaded, the query after --scaled and as given
+    src = _Loaded(db, rows, query, given_mh)
+    return qmh, sset, meta, src
+
+
+class _Loaded:
+    "The loaded side of a search: row r of the compared set is signature ``rows[r]`` of ``db``."
+    def __init__(self, db, rows, query, given_mh):
+        self.db, self.rows, self.query, self.given_mh = db, rows, query, given_mh
+
+    def signatures(self, rows):
+        "the signatures behind rows of the compared set, as loaded (not downsampled), in the given order"
+        return self.db.signatures(self.rows[np.asarray(rows, dtype=np.int64)]) if len(rows) else []
+
+
+_COLLECTION_TARGETS = ((".zip", "a .zip collection"), (".sqldb", "a SQLite database"), ("/", "a directory"))
+
+
+def _check_sig_targets(*targets):
+    """Signature outputs go to a .sig file (gzip JSON for a path ending in .gz) or to stdout for ``-``, as the reference's
+    SaveSignatures_SigFile writes them (save_load.py:406-445); collections are refused before anything is loaded."""
+    for t in targets:
+        for suffix, what in _COLLECTION_TARGETS:
+            if t and t.endswith(suffix):
+                print(f"ERROR: cannot save signatures to {what} ('{t}'); write a .sig or .sig.gz file, or - for stdout",
+                      file=sys.stderr)
+                raise SystemExit(-1)
+
+
+def _save_sigs(path, sigs):
+    from .signature import save_signatures_to_json
+    if path == "-":
+        save_signatures_to_json(sigs, sys.stdout)
+        sys.stdout.flush()
+        return
+    gz = path.endswith(".gz")
+    with open(path, "wb" if gz else "w", encoding=None if gz else "utf-8") as fp:
+        save_signatures_to_json(sigs, fp, compression=1 if gz else 0)
+
+
+def _sketch_of(template, hashes, abund_from=None):
+    """A sketch with ``template``'s parameters holding ``hashes`` (sorted, unique).  With ``abund_from`` (a sketch with
+    abundances that holds every hash): ``flat.inflate(abund_from)`` -- the abundances taken from it, and its max_hash
+    kept, because the reference's inflate discards its own downsample (minhash.py:1071-1087) -- built from arrays."""
+    from ._ffi import rustcall
+    from ._lowlevel import ffi, lib
+    hashes = np.ascontiguousarray(hashes, dtype=np.uint64)
+    if abund_from is None:
+        mh = template._blank_like(track_abundance=False)
+        mh.add_many(hashes)
+        return mh
+    mh = abund_from._blank_like()
+    src = abund_from._mins_array()
+    abunds = np.ascontiguousarray(abund_from._abunds_array()[np.searchsorted(src, hashes)], dtype=np.uint64)
+    rustcall(lib.kmerminhash_set_abundances, mh._get_objptr(), ffi.cast("uint64_t *", hashes.ctypes.data),
+             ffi.cast("uint64_t *", abunds.ctypes.data), len(hashes), True)
+    return mh
 
 
 class Command_B200Gather(CommandLinePlugin):
@@ -270,22 +327,107 @@ class Command_B200Gather(CommandLinePlugin):
         p.add_argument("--ignore-abundance", action="store_true")
         p.add_argument("--estimate-ani-ci", action="store_true")
         p.add_argument("-o", "--output", default=None, help="CSV of the matches")
+        p.add_argument("--save-matches", default=None, help="save the picked signatures (.sig, .sig.gz or -)")
+        p.add_argument("--save-prefetch", default=None, help="save the signatures of the prefetch stage")
+        p.add_argument("--save-prefetch-csv", default=None, help="prefetch CSV of the prefetch stage")
+        p.add_argument("--output-unassigned", default=None, help="save the query hashes no match took")
 
     def main(self, args):
         super().main(args)
         from .gather import gather_databases, write_gather_csv
-        qmh, sset, meta = _load_query_and_db(args)
-        meta.pop("match_orig")
-        meta.pop("groups")
+        _check_sig_targets(args.save_matches, args.save_prefetch, args.output_unassigned)
+        qmh, sset, meta, src = _load_query_and_db(args)
+        match_orig = meta.pop("match_orig")
+        groups = meta.pop("groups")
+        stats = {}
         rows = gather_databases(qmh, sset, threshold_bp=args.threshold_bp, ignore_abundance=args.ignore_abundance,
-                                estimate_ani_ci=args.estimate_ani_ci, **meta)
+                                estimate_ani_ci=args.estimate_ani_ci, stats=stats, **meta)
+        if args.save_prefetch or args.save_prefetch_csv:
+            self._save_prefetch(args, qmh, sset, meta, match_orig, groups, stats, src)
+        if args.save_matches:                               # the picks, in pick order (commands.py:1043-1045)
+            _notify(args, f"saving all matches to '{args.save_matches}'")
         for g in rows:
             _notify(args, f"{g.intersect_bp / 1e3:9.1f} kbp {g.f_orig_query * 100:6.1f}% {g.f_match * 100:6.1f}%  {g.name}")
+        if args.save_matches and rows:                      # nothing picked: the reference's empty saver writes no file
+            # the counter of a database holds the last of the signatures that share an md5 (index/__init__.py:777-794)
+            last = {}
+            for r in self._passing(stats).tolist():
+                last[(groups[r], meta["md5s"][r])] = r
+            _save_sigs(args.save_matches, src.signatures([last.get((groups[g.row], meta["md5s"][g.row]), g.row)
+                                                          for g in rows]))
         _notify(args, f"found {len(rows)} matches total")
         if args.output and rows:                            # no matches: the reference leaves without creating the file
             with open(args.output, "w", newline="") as fp:
                 write_gather_csv(rows, fp, estimate_ani_ci=args.estimate_ani_ci)
+        if args.output_unassigned:
+            self._save_unassigned(args, qmh, sset, rows, stats, src)
         return 0
+
+    @staticmethod
+    def _passing(stats):
+        "rows of the compared set at or above the prefetch threshold (none when the threshold is unattainable)"
+        if stats["counts0"] is None:                        # no database yields a counter (commands.py:909-914)
+            return np.zeros(0, dtype=np.int64)
+        return np.nonzero(stats["counts0"].astype(np.int64) >= max(1, stats["min_count"]))[0]
+
+    @classmethod
+    def _prefetch_rows(cls, groups, md5s, stats):
+        """Rows of the prefetch stage as the reference's save_prefetch holds them (commands.py:894-922): database argument
+        after argument, and inside one the rows at or above the threshold collapsed by md5 -- CounterGather.add keys a
+        dict by md5, so the entry keeps the first duplicate's place and the last one's signature (index/__init__.py:777-794)."""
+        by_group = {}
+        for r in cls._passing(stats).tolist():
+            by_group.setdefault(groups[r], {})[md5s[r]] = r
+        return [r for k in sorted(by_group) for r in by_group[k].values()]
+
+    def _save_prefetch(self, args, qmh, sset, meta, match_orig, groups, stats, src):
+        from .gather import prefetch_database, write_prefetch_csv
+        rows = self._prefetch_rows(groups, meta["md5s"], stats)
+        if args.save_prefetch:
+            _save_sigs(args.save_prefetch, src.signatures(rows))
+        if args.save_prefetch_csv:
+            res = []
+            if rows:                                        # PrefetchResult of the flattened query (commands.py:924-934)
+                pm = {k: v for k, v in meta.items() if k != "locations"}
+                flat = qmh.flatten() if qmh.track_abundance else qmh
+                by_row = {d["row"]: d for d in prefetch_database(flat, sset, args.threshold_bp, counts=stats["counts0"],
+                                                                 estimate_ani_ci=args.estimate_ani_ci,
+                                                                 match_orig=match_orig, **pm)}
+                res = [by_row[r] for r in rows]
+            with open(args.save_prefetch_csv, "w", newline="") as fp:
+                write_prefetch_csv(res, fp, estimate_ani_ci=args.estimate_ani_ci)
+
+    @classmethod
+    def _save_unassigned(cls, args, qmh, sset, rows, stats, src):
+        """The query hashes that no pick took: the remaining query plus the prefetch's noident hashes
+        (commands.py:1094-1112), named as GatherDatabases names its query (search.py:826-827,918-920).  Without a pick
+        that is the whole query at its own scaled (after --scaled).  After a pick the remaining query is at the comparison
+        scaled and noident at the query's; when a database coarser than the query makes these differ, the reference's
+        `remaining_mh += noident_mh` fails on the two scaled values, and so does this (an empty noident is not merged)."""
+        from . import batch as B
+        from .signature import SourmashSignature
+        noident = np.zeros(0, dtype=np.uint64)
+        if rows:
+            q, left = stats["q_hashes"], stats["q_hashes"][stats["alive"]]
+            if qmh.scaled != src.query.minhash.scaled:
+                full = src.query.minhash._mins_array()       # q is its prefix: the hashes <= the comparison's max_hash
+                held = B.query_covered(q, sset, cls._passing(stats))
+                noident = np.concatenate([q[~held], full[len(q):]])
+        else:
+            left = src.query.minhash._mins_array()
+        if not len(left) and not len(noident):
+            _notify(args, "no unassigned hashes to save with --output-unassigned!")
+            return
+        _notify(args, f"saving unassigned hashes to '{args.output_unassigned}'")
+        if len(noident):                                    # two max_hash values: merge raises, as in the reference
+            _sketch_of(qmh, left).merge(_sketch_of(src.query.minhash, noident))
+        abund = qmh.track_abundance and not args.ignore_abundance
+        mh = _sketch_of(qmh if rows else src.query.minhash, left, abund_from=src.query.minhash if abund else None)
+        if rows:
+            sig = SourmashSignature(mh)
+        else:
+            sig = SourmashSignature(mh, name=src.query.name or "", filename=src.query.filename or "")
+        _save_sigs(args.output_unassigned, [sig])
 
 
 class Command_B200Prefetch(CommandLinePlugin):
@@ -300,23 +442,59 @@ class Command_B200Prefetch(CommandLinePlugin):
         p.add_argument("--threshold-bp", type=float, default=50000.0)
         p.add_argument("--estimate-ani-ci", action="store_true")
         p.add_argument("-o", "--output", default=None, help="CSV of the matches")
+        p.add_argument("--save-matches", default=None, help="save the matching database signatures (.sig, .sig.gz or -)")
+        p.add_argument("--save-matching-hashes", default=None, help="save the query hashes found in the matches")
+        p.add_argument("--save-unmatched-hashes", default=None, help="save the query hashes no match holds")
 
     def main(self, args):
         super().main(args)
         from .gather import prefetch_database, write_prefetch_csv
+        _check_sig_targets(args.save_matches, args.save_matching_hashes, args.save_unmatched_hashes)
         if args.output:
             open(args.output, "w").close()                  # created before the search, as in the reference (empty if it fails)
-        qmh, sset, meta = _load_query_and_db(args)
+        qmh, sset, meta, src = _load_query_and_db(args)
         meta.pop("locations")                              # prefetch reports the filename stored in the match (match_filename)
         meta.pop("groups")
         if qmh.track_abundance:                             # prefetch works on the flattened query (commands.py: prefetch)
             qmh = qmh.flatten()
+        if args.save_matches:
+            _notify(args, f"saving all matching database signatures to '{args.save_matches}'")
         res = prefetch_database(qmh, sset, args.threshold_bp, estimate_ani_ci=args.estimate_ani_ci, **meta)
         _notify(args, f"total of {len(res)} matching signatures")
+        if args.save_matches:                               # every match as loaded, in CSV order (commands.py:1631)
+            _save_sigs(args.save_matches, src.signatures([d["row"] for d in res]))
         if args.output:
             with open(args.output, "w", newline="") as fp:
                 write_prefetch_csv(res, fp, estimate_ani_ci=args.estimate_ani_ci)
+        if args.save_matching_hashes or args.save_unmatched_hashes:
+            self._save_hashes(args, qmh, sset, [d["row"] for d in res], src)
         return 0
+
+    @staticmethod
+    def _save_hashes(args, qmh, sset, rows, src):
+        """The query hashes the matches hold ("known") and the rest ("unknown"), the reference's ident_mh / noident_mh
+        (commands.py:1602-1622,1674-1712): the flattened query at the comparison's scaled, split by one device pass over
+        the matches; with no match, at the query's own scaled (after --scaled), all of it unknown."""
+        from . import batch as B
+        from .signature import SourmashSignature
+        if rows:
+            template = qmh
+            q = qmh._mins_array()
+            covered = B.query_covered(q, sset, rows)
+        else:
+            template = src.query.minhash.flatten()
+            q = template._mins_array()
+            covered = np.zeros(len(q), dtype=bool)
+        given = src.given_mh if src.given_mh.track_abundance else None
+        name = src.query.name
+        for path, mask, tag, what in ((args.save_matching_hashes, covered, "known", "matched"),
+                                      (args.save_unmatched_hashes, ~covered, "unknown", "unmatched")):
+            if not path:
+                continue
+            hashes = q[mask]
+            _notify(args, f"saving {len(hashes)} {what} hashes to '{path}'")
+            mh = _sketch_of(template, hashes, abund_from=given)
+            _save_sigs(path, [SourmashSignature(mh, name=f"{name}-{tag}" if name else "")])
 
 
 class Command_B200Search(CommandLinePlugin):
@@ -336,12 +514,14 @@ class Command_B200Search(CommandLinePlugin):
         p.add_argument("-n", "--num-results", type=int, default=3, help="matches to print (0: all; the CSV has all)")
         p.add_argument("--estimate-ani-ci", action="store_true")
         p.add_argument("-o", "--output", default=None, help="CSV of the matches")
+        p.add_argument("--save-matches", default=None, help="save the signature of every match (.sig, .sig.gz or -)")
 
     def main(self, args):
         super().main(args)
         from .gather import write_search_csv
         if args.containment and args.max_containment:
             raise ValueError("--containment and --max-containment are mutually exclusive")
+        _check_sig_targets(args.save_matches)
         res = self._abundance_search(args)                 # None: a flat query, or --ignore-abundance
         if res is None:
             res = self._flat_search(args)
@@ -354,6 +534,9 @@ class Command_B200Search(CommandLinePlugin):
         if args.output:
             with open(args.output, "w", newline="") as fp:
                 write_search_csv(res, fp, estimate_ani_ci=args.estimate_ani_ci)
+        if args.save_matches:                                      # every result row's match, in CSV order (commands.py:737-743)
+            _notify(args, f"saving all matched signatures to \"{args.save_matches}\"")
+            _save_sigs(args.save_matches, [d["match"] for d in res])
         return 0
 
     @staticmethod
@@ -385,17 +568,21 @@ class Command_B200Search(CommandLinePlugin):
             raise SystemExit(-1)
         found.sort(key=lambda x: -x[0])
         return [{"similarity": score, "md5": match.md5sum(), "filename": location, "name": match.name,
-                 "query_filename": query.filename, "query_name": query.name, "query_md5": query.md5sum()[:8], "ani": None}
+                 "query_filename": query.filename, "query_name": query.name, "query_md5": query.md5sum()[:8], "ani": None,
+                 "match": match}
                 for score, match, location in found]
 
     @staticmethod
     def _flat_search(args):
         from .gather import search_database
-        qmh, sset, meta = _load_query_and_db(args)
+        qmh, sset, meta, src = _load_query_and_db(args)
         meta.pop("match_orig")
         res = search_database(qmh.flatten() if qmh.track_abundance else qmh, sset, threshold=args.threshold,
                               do_containment=args.containment, do_max_containment=args.max_containment,
                               best_only=args.best_only, estimate_ani_ci=args.estimate_ani_ci, **meta)   # `groups`: one database per argument
+        if args.save_matches:
+            for d, match in zip(res, src.signatures([d["row"] for d in res])):
+                d["match"] = match
         return res
 
 
