@@ -482,6 +482,42 @@ const uint64_t *smb_combined_hashes(const SmbCombined *c);                /* len
 const uint64_t *smb_combined_abunds(const SmbCombined *c);                /* len, or null */
 void smb_combined_free(SmbCombined *c);
 
+/* Taxonomic classification against LCA databases (`lca classify`, `lca summarize`; the reference's per-hash loop is
+ * lca/lca_utils.py:186-225).
+ * smb_lca_parse_hashvals: the "hashval_to_idx" member of an LCA database's JSON text as one (hash, idx) pair per listed
+ * idx, in file order, and the byte span [begin, end) of that member's value (-1, -1 when absent).  Host only.
+ * smb_lca_table_build: the taxonomy trie is parent[] / depth[] over n_nodes nodes, node 0 the root at depth 0, and
+ * parent[i] < i with depth[i] = depth[parent[i]] + 1.  The n (hash, node) pairs are every database's (node
+ * 0xffffffff: the pair contributes nothing, as an idx without a lineage).  Every distinct hash <= max_hash that has
+ * a node gets the node the reference's tree walk (build_tree + find_lca) gives for its lineages: the deepest node
+ * when they lie on one root path, else the node where they branch.  Node indices, the trie's shape and its size are
+ * checked before any launch; no pairs: an empty table, no launch.
+ * smb_lca_counts: for every query (row) of `queries`, every distinct LCA node of its hashes found in the table, with
+ * the number of those hashes (use_abunds: the sum of their abundances) and the smallest position in the row of a
+ * hash with that node.  Rows ordered by (query, node).  Offsets that do not start at 0 or decrease are refused; an
+ * empty batch or an empty table gives no rows and no launch. */
+typedef struct SmbLcaHashvals SmbLcaHashvals;
+SmbLcaHashvals *smb_lca_parse_hashvals(const char *text, uintptr_t len);
+uintptr_t smb_lca_hashvals_len(const SmbLcaHashvals *h);
+const uint64_t *smb_lca_hashvals_hashes(const SmbLcaHashvals *h);        /* len */
+const uint32_t *smb_lca_hashvals_idx(const SmbLcaHashvals *h);           /* len */
+void smb_lca_hashvals_span(const SmbLcaHashvals *h, int64_t *begin, int64_t *end);
+void smb_lca_hashvals_free(SmbLcaHashvals *h);
+typedef struct SmbLcaTable SmbLcaTable;
+SmbLcaTable *smb_lca_table_build(const uint64_t *hashes, const uint32_t *nodes, uintptr_t n, const uint32_t *parent,
+                                 const uint8_t *depth, uint32_t n_nodes, uint64_t max_hash);
+uintptr_t smb_lca_table_len(const SmbLcaTable *t);                        /* distinct hashes with a node */
+void smb_lca_table_copy(const SmbLcaTable *t, uint64_t *hashes, uint32_t *lca);   /* len each, hashes ascending */
+void smb_lca_table_free(SmbLcaTable *t);
+typedef struct SmbLcaCounts SmbLcaCounts;
+SmbLcaCounts *smb_lca_counts(const SmbLcaTable *t, const SmbSketchSet *queries, bool use_abunds);
+uintptr_t smb_lca_counts_len(const SmbLcaCounts *c);
+const uint32_t *smb_lca_counts_query(const SmbLcaCounts *c);             /* len each */
+const uint32_t *smb_lca_counts_node(const SmbLcaCounts *c);
+const uint64_t *smb_lca_counts_count(const SmbLcaCounts *c);
+const uint64_t *smb_lca_counts_first(const SmbLcaCounts *c);
+void smb_lca_counts_free(SmbLcaCounts *c);
+
 /* Signature objects straight from a sketch set (the tail of _compute_individual,
  * command_sketch.py:770-789): signature g owns rows [g * n_ksizes, (g + 1) * n_ksizes); ksizes
  * are the ABI values.  Array freed with signatures_array_free, objects with signature_free. */

@@ -395,6 +395,94 @@ def combine(sset, op, num=0):
         lib.smb_combined_free(p)
 
 
+LCA_NO_NODE = 0xFFFFFFFF
+
+
+def lca_parse_hashvals(text):
+    """The "hashval_to_idx" member of an LCA database's JSON text (bytes), parsed natively: ``(hashes, idx, span)``,
+    one uint64 hash and one uint32 idx per listed idx in file order, and the byte span ``(begin, end)`` of the member's
+    value (``(-1, -1)`` when the document has none).  Raises on malformed JSON inside the member."""
+    buf = ffi.from_buffer(text)
+    p = rustcall(lib.smb_lca_parse_hashvals, buf, len(text))
+    try:
+        n = int(lib.smb_lca_hashvals_len(p))
+        h = np.frombuffer(ffi.buffer(lib.smb_lca_hashvals_hashes(p), n * 8), dtype=np.uint64).copy() if n else \
+            np.zeros(0, np.uint64)
+        ix = np.frombuffer(ffi.buffer(lib.smb_lca_hashvals_idx(p), n * 4), dtype=np.uint32).copy() if n else \
+            np.zeros(0, np.uint32)
+        b, e = ffi.new("int64_t *"), ffi.new("int64_t *")
+        lib.smb_lca_hashvals_span(p, b, e)
+        return h, ix, (int(b[0]), int(e[0]))
+    finally:
+        lib.smb_lca_hashvals_free(p)
+
+
+class LcaTable:
+    """The LCA node of every distinct database hash, resident on the GPU (``lca_table``)."""
+
+    def __init__(self, ptr):
+        self._ptr = ptr
+
+    def __del__(self):
+        p, self._ptr = getattr(self, "_ptr", None), None
+        if p and lib is not None:
+            lib.smb_lca_table_free(p)
+
+    def __len__(self):
+        return int(lib.smb_lca_table_len(self._ptr))
+
+    def to_host(self):
+        "(hashes ascending, lca nodes) as numpy arrays"
+        n = len(self)
+        h, lca = np.zeros(n, np.uint64), np.zeros(n, np.uint32)
+        rustcall(lib.smb_lca_table_copy, self._ptr, _ptr(h, "uint64_t *"), _ptr(lca, "uint32_t *"))
+        return h, lca
+
+
+def lca_table(hashes, nodes, parent, depth, max_hash=2**64 - 1):
+    """Fold the (hash, trie node) pairs of every database into one LCA node per distinct hash, on the device.  The trie
+    is ``parent`` / ``depth`` (node 0 the root; ``parent[i] < i``); a node of ``LCA_NO_NODE`` contributes nothing, and
+    hashes above ``max_hash`` are cut.  The node of a hash is the one the reference's tree walk gives for its lineages:
+    the deepest when they lie on one root path, else the node where they branch."""
+    h = _u64(hashes)
+    nd = np.ascontiguousarray(nodes, dtype=np.uint32)
+    par = np.ascontiguousarray(parent, dtype=np.uint32)
+    dep = np.ascontiguousarray(depth, dtype=np.uint8)
+    if len(h) != len(nd):
+        raise ValueError("hashes and nodes differ in length")
+    if len(par) != len(dep):
+        raise ValueError("parent and depth differ in length")
+    return LcaTable(rustcall(lib.smb_lca_table_build, _ptr(h, "uint64_t *"), _ptr(nd, "uint32_t *"), len(h),
+                             _ptr(par, "uint32_t *"), _ptr(dep, "uint8_t *"), len(par), int(max_hash)))
+
+
+def lca_counts(table, query_hashes, offsets=None, weights=None):
+    """Every distinct (query, LCA node) of a batch of queries' hashes found in ``table``: ``(query, node, count,
+    first)`` as numpy arrays ordered by (query, node).  ``count`` sums the weights of the hashes (1 each, or the
+    query's abundances), ``first`` is the smallest position in the query of a hash with that node.  The queries are a
+    CSR (``query_hashes``, ``offsets``, optional ``weights`` parallel to the hashes) or a resident ``SketchSet``, with
+    ``weights=True`` to weight by its abundances."""
+    if isinstance(query_hashes, SketchSet):
+        sset, use = query_hashes, bool(weights)
+    else:
+        h, off = _u64(query_hashes), _u64(offsets)
+        if len(off) == 0 or int(off[-1]) != len(h) or (weights is not None and len(weights) != len(h)):
+            raise ValueError("query offsets must end at the number of hashes, and weights match the hashes")
+        sset = SketchSet.from_host(h, off, weights)
+        use = weights is not None
+    p = rustcall(lib.smb_lca_counts, table._ptr, sset._ptr, use)
+    try:
+        n = int(lib.smb_lca_counts_len(p))
+
+        def take(fn, dtype):
+            return np.frombuffer(ffi.buffer(fn(p), n * np.dtype(dtype).itemsize), dtype=dtype).copy() if n else \
+                np.zeros(0, dtype)
+        return (take(lib.smb_lca_counts_query, np.uint32), take(lib.smb_lca_counts_node, np.uint32),
+                take(lib.smb_lca_counts_count, np.uint64), take(lib.smb_lca_counts_first, np.uint64))
+    finally:
+        lib.smb_lca_counts_free(p)
+
+
 def gather(query, db, threshold=1, max_rounds=None):
     """Iterative min-set-cover; returns (match_ids, intersect_sizes) in pick order."""
     q = _u64(query)

@@ -3255,6 +3255,131 @@ const uint64_t* smb_combined_hashes(const SmbCombined* c) { return c->hashes.dat
 const uint64_t* smb_combined_abunds(const SmbCombined* c) { return c->has_abunds ? c->abunds.data() : nullptr; }
 void smb_combined_free(SmbCombined* c) { delete c; }
 
+// `lca classify` / `lca summarize` (lca/lca_utils.py:186-225): the LCA node of every database hash, found once per
+// command (lca_table_build), then per batch of queries the distinct (query, node) of their hashes with summed weights
+// and first positions (lca_counts).  Only those rows come back to the host.
+struct SmbLcaHashvals {
+    std::vector<uint64_t> hashes;
+    std::vector<uint32_t> idx;
+    int64_t begin = -1, end = -1;
+};
+
+SmbLcaHashvals* smb_lca_parse_hashvals(const char* text, uintptr_t len) {
+    return guarded<SmbLcaHashvals*>([&]() -> SmbLcaHashvals* {
+        auto r = std::make_unique<SmbLcaHashvals>();
+        std::string err = smb::parse_lca_hashvals(text, len, r->hashes, r->idx, &r->begin, &r->end);
+        if (!err.empty()) fail(SOURMASH_ERROR_CODE_SERDE_ERROR, err);
+        return r.release();
+    });
+}
+uintptr_t smb_lca_hashvals_len(const SmbLcaHashvals* h) { return h->hashes.size(); }
+const uint64_t* smb_lca_hashvals_hashes(const SmbLcaHashvals* h) { return h->hashes.data(); }
+const uint32_t* smb_lca_hashvals_idx(const SmbLcaHashvals* h) { return h->idx.data(); }
+void smb_lca_hashvals_span(const SmbLcaHashvals* h, int64_t* begin, int64_t* end) { *begin = h->begin; *end = h->end; }
+void smb_lca_hashvals_free(SmbLcaHashvals* h) { delete h; }
+
+struct SmbLcaTable {
+    DevBuf<uint64_t> hashes;
+    DevBuf<uint32_t> lca, parent;
+    DevBuf<uint8_t> depth;
+    uint64_t n = 0;
+    uint32_t n_nodes = 0;
+};
+
+SmbLcaTable* smb_lca_table_build(const uint64_t* hashes, const uint32_t* nodes, uintptr_t n, const uint32_t* parent,
+                                 const uint8_t* depth, uint32_t n_nodes, uint64_t max_hash) {
+    return guarded<SmbLcaTable*>([&]() -> SmbLcaTable* {
+        if (n_nodes == 0) fail(SOURMASH_ERROR_CODE_MSG, "the taxonomy trie has no nodes (node 0 is the root)");
+        if (n_nodes == smb::LCA_NO_NODE) fail(SOURMASH_ERROR_CODE_MSG, "the taxonomy trie has too many nodes");
+        if (depth[0] != 0) fail(SOURMASH_ERROR_CODE_MSG, "node 0 must be the root, at depth 0");
+        for (uint32_t i = 1; i < n_nodes; ++i)
+            if (parent[i] >= i || depth[i] != depth[parent[i]] + 1)
+                fail(SOURMASH_ERROR_CODE_MSG, "trie node " + std::to_string(i) + " needs a parent below it, one rank up");
+        for (uintptr_t i = 0; i < n; ++i)
+            if (nodes[i] >= n_nodes && nodes[i] != smb::LCA_NO_NODE)
+                fail(SOURMASH_ERROR_CODE_MSG, "node " + std::to_string(nodes[i]) + " out of range for a trie of " +
+                                                  std::to_string(n_nodes) + " nodes");
+        if (n > 0x7fffffffull) fail(SOURMASH_ERROR_CODE_MSG, "LCA table too large (more than 2^31 - 1 pairs)");
+        auto t = std::make_unique<SmbLcaTable>();
+        t->n_nodes = n_nodes;
+        if (n == 0) return t.release();
+        cudaStream_t s = need_gpu();
+        uint64_t max_key = 0;
+        for (uintptr_t i = 0; i < n; ++i) max_key = std::max(max_key, hashes[i]);
+        t->parent.alloc(n_nodes, s); t->parent.upload(parent, n_nodes);
+        t->depth.alloc(n_nodes, s); t->depth.upload(depth, n_nodes);
+        DevBuf<uint64_t> d_h(n, s);
+        DevBuf<uint32_t> d_nodes(n, s);
+        d_h.upload(hashes, n);
+        d_nodes.upload(nodes, n);
+        uint64_t* out_h = nullptr;
+        uint32_t* out_lca = nullptr;
+        if (t_profiling) t_timer_hash.begin(s);
+        CK(smb::lca_table_build(d_h.p, d_nodes.p, n, max_hash, max_key, t->parent.p, t->depth.p, &out_h, &out_lca,
+                                &t->n, s));
+        if (t_profiling) t_timer_hash.end(s);
+        t->hashes.p = out_h; t->hashes.n = n; t->hashes.s = s;
+        t->lca.p = out_lca; t->lca.n = n; t->lca.s = s;
+        return t.release();
+    });
+}
+uintptr_t smb_lca_table_len(const SmbLcaTable* t) { return t->n; }
+void smb_lca_table_copy(const SmbLcaTable* t, uint64_t* hashes, uint32_t* lca) {
+    guarded_void([&] {
+        if (t->n == 0) return;
+        t->hashes.download(hashes, t->n);
+        t->lca.download(lca, t->n);
+        sync(t->hashes.s);
+    });
+}
+void smb_lca_table_free(SmbLcaTable* t) { delete t; }
+
+struct SmbLcaCounts {
+    std::vector<uint32_t> query, node;
+    std::vector<uint64_t> count, first;
+};
+
+SmbLcaCounts* smb_lca_counts(const SmbLcaTable* t, const SmbSketchSet* queries, bool use_abunds) {
+    return guarded<SmbLcaCounts*>([&]() -> SmbLcaCounts* {
+        const std::vector<uint64_t>& off = queries->h_off;
+        if (queries->n_rows >= smb::LCA_NO_NODE) fail(SOURMASH_ERROR_CODE_MSG, "too many queries in one batch");
+        if (!off.empty() && off[0] != 0) fail(SOURMASH_ERROR_CODE_MSG, "query offsets must start at 0");
+        for (size_t i = 1; i < off.size(); ++i)
+            if (off[i] < off[i - 1]) fail(SOURMASH_ERROR_CODE_MSG, "query offsets decrease at " + std::to_string(i));
+        if (use_abunds && !queries->d_abunds) fail(SOURMASH_ERROR_CODE_MSG, "the queries carry no abundances");
+        const uint64_t Tq = queries->total();
+        if (Tq > 0x7fffffffull) fail(SOURMASH_ERROR_CODE_MSG, "query batch too large (more than 2^31 - 1 hashes)");
+        auto r = std::make_unique<SmbLcaCounts>();
+        if (Tq == 0 || t->n == 0) return r.release();
+        cudaStream_t s = need_gpu();
+        uint32_t *d_q = nullptr, *d_node = nullptr;
+        uint64_t *d_w = nullptr, *d_first = nullptr, n = 0;
+        if (t_profiling) t_timer_hash.begin(s);
+        CK(smb::lca_counts(t->hashes.p, t->lca.p, t->n, queries->d_hashes, queries->d_off, (uint32_t)queries->n_rows,
+                           Tq, use_abunds ? queries->d_abunds : nullptr, &d_q, &d_node, &d_w, &d_first, &n, s));
+        if (t_profiling) t_timer_hash.end(s);
+        DevBuf<uint32_t> b_q, b_node;                                  // owned from here on, freed on every path
+        DevBuf<uint64_t> b_w, b_first;
+        b_q.p = d_q; b_q.n = Tq; b_q.s = s;
+        b_node.p = d_node; b_node.n = Tq; b_node.s = s;
+        b_w.p = d_w; b_w.n = Tq; b_w.s = s;
+        b_first.p = d_first; b_first.n = Tq; b_first.s = s;
+        r->query.resize(n); r->node.resize(n); r->count.resize(n); r->first.resize(n);
+        b_q.download(r->query.data(), n);
+        b_node.download(r->node.data(), n);
+        b_w.download(r->count.data(), n);
+        b_first.download(r->first.data(), n);
+        sync(s);
+        return r.release();
+    });
+}
+uintptr_t smb_lca_counts_len(const SmbLcaCounts* c) { return c->query.size(); }
+const uint32_t* smb_lca_counts_query(const SmbLcaCounts* c) { return c->query.data(); }
+const uint32_t* smb_lca_counts_node(const SmbLcaCounts* c) { return c->node.data(); }
+const uint64_t* smb_lca_counts_count(const SmbLcaCounts* c) { return c->count.data(); }
+const uint64_t* smb_lca_counts_first(const SmbLcaCounts* c) { return c->first.data(); }
+void smb_lca_counts_free(SmbLcaCounts* c) { delete c; }
+
 // signatures straight from a sketch set (the tail of _compute_individual, command_sketch.py:770-789):
 // signature s gets rows [s * n_ksizes, (s + 1) * n_ksizes) of `set` as its sketches
 SourmashSignature** smb_signatures_from_sketchset(const SmbSketchSet* set, const uint32_t* ksizes,

@@ -39,6 +39,7 @@
 #include "tile_kernels.cuh"
 #include "pair_kernels.cuh"
 #include "sketch_combine.cuh"
+#include "lca_kernels.cuh"
 #include "angular_search.cuh"
 
 namespace smb {
@@ -1008,6 +1009,109 @@ cudaError_t sketchset_combine(const u64* h, const u64* abund, u64 n_rows, u64 T,
         return e;
     }
     *out_h = oh; *out_v = ov; *out_n = n;
+    return cudaSuccess;
+}
+
+// ------------------------------------------------------------------------------------
+// Taxonomic LCA (lca_kernels.cuh).  The table build: a sort of the (hash, node) pairs, the fold, a scan and a scatter,
+// with one readback (the number of distinct hashes).  The counts: the probe, a sort of (query << 32 | node, element),
+// the run pass, a scan and a scatter, with one readback (the number of rows).  Each output is allocated at its bound
+// (the input length), so that readback is the only one.
+// ------------------------------------------------------------------------------------
+static cudaError_t exclusive_sum_u32(const u32* in, u32* out, u64 n, cudaStream_t s) {
+    size_t bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, (int)n, s);
+    void* tmp = nullptr;
+    cudaError_t e = cudaMallocAsync(&tmp, bytes ? bytes : 16, s);
+    if (e != cudaSuccess) return e;
+    cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, (int)n, s);
+    cudaFreeAsync(tmp, s);
+    count_launches(1);
+    return cudaGetLastError();
+}
+
+// reads *d_count back; on failure frees the n_out arrays of out[]
+static cudaError_t read_count(const unsigned long long* d_count, u64* n, void** out, int n_out, cudaStream_t s) {
+    unsigned long long c = 0;
+    cudaMemcpyAsync(&c, d_count, sizeof c, cudaMemcpyDeviceToHost, s);
+    cudaError_t e;
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) {
+        for (int i = 0; i < n_out; ++i) if (out[i]) cudaFreeAsync(out[i], s);
+        return e;
+    }
+    *n = c;
+    return cudaSuccess;
+}
+
+cudaError_t lca_table_build(const u64* h, const u32* nodes, u64 n, u64 max_hash, u64 max_key, const u32* parent,
+                            const u8* depth, u64** out_h, u32** out_lca, u64* out_n, cudaStream_t s) {
+    *out_h = nullptr; *out_lca = nullptr; *out_n = 0;
+    if (n == 0) return cudaSuccess;
+    if (n > 0x7fffffffull) return cudaErrorInvalidValue;
+    JoinScratch scratch(s);
+    cudaError_t e;
+    u64* keys = nullptr;
+    u32 *nodes_sorted = nullptr, *flag = nullptr, *pos = nullptr, *lca = nullptr;
+    unsigned long long* d_count = nullptr;
+    if ((e = scratch.alloc((void**)&keys, n * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&nodes_sorted, n * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&flag, n * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&pos, n * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&lca, n * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&d_count, sizeof(unsigned long long))) != cudaSuccess) return e;
+    if ((e = sort_hash_pairs(h, keys, nodes, nodes_sorted, n, max_key, s)) != cudaSuccess) return e;
+    const unsigned blocks = (unsigned)std::min<u64>((n + 255) / 256, (u64)SMB_SMS * 32);
+    lca_fold_kernel<<<blocks, 256, 0, s>>>(keys, nodes_sorted, n, max_hash, parent, depth, flag, lca);
+    count_launches(1);
+    if ((e = exclusive_sum_u32(flag, pos, n, s)) != cudaSuccess) return e;
+    void* out[2] = {};
+    if ((e = cudaMallocAsync(&out[0], n * sizeof(u64), s)) != cudaSuccess) return e;
+    if ((e = cudaMallocAsync(&out[1], n * sizeof(u32), s)) != cudaSuccess) { cudaFreeAsync(out[0], s); return e; }
+    lca_scatter_kernel<<<blocks, 256, 0, s>>>(keys, lca, flag, pos, n, (u64*)out[0], (u32*)out[1], d_count);
+    count_launches(1);
+    if ((e = read_count(d_count, out_n, out, 2, s)) != cudaSuccess) return e;
+    *out_h = (u64*)out[0]; *out_lca = (u32*)out[1];
+    return cudaSuccess;
+}
+
+cudaError_t lca_counts(const u64* t_h, const u32* t_lca, u64 n_t, const u64* qh, const u64* q_off, u32 n_q, u64 Tq,
+                       const u64* abund, u32** out_q, u32** out_node, u64** out_w, u64** out_first, u64* out_n,
+                       cudaStream_t s) {
+    *out_q = *out_node = nullptr; *out_w = *out_first = nullptr; *out_n = 0;
+    if (Tq == 0 || n_t == 0 || n_q == 0) return cudaSuccess;
+    if (Tq > 0x7fffffffull) return cudaErrorInvalidValue;
+    JoinScratch scratch(s);
+    cudaError_t e;
+    u64 *key = nullptr, *key_sorted = nullptr, *weight = nullptr;
+    u32 *idx = nullptr, *idx_sorted = nullptr, *flag = nullptr, *pos = nullptr;
+    unsigned long long* d_count = nullptr;
+    if ((e = scratch.alloc((void**)&key, Tq * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&key_sorted, Tq * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&weight, Tq * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&idx, Tq * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&idx_sorted, Tq * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&flag, Tq * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&pos, Tq * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&d_count, sizeof(unsigned long long))) != cudaSuccess) return e;
+    const unsigned blocks = (unsigned)std::min<u64>((Tq + 255) / 256, (u64)SMB_SMS * 32);
+    lca_probe_kernel<<<blocks, 256, 0, s>>>(qh, q_off, n_q, Tq, t_h, t_lca, n_t, key, idx); count_launches(1);
+    const u64 miss_key = (u64)n_q << 32;
+    if ((e = sort_hash_pairs(key, key_sorted, idx, idx_sorted, Tq, miss_key, s)) != cudaSuccess) return e;
+    lca_count_runs_kernel<<<blocks, 256, 0, s>>>(key_sorted, idx_sorted, Tq, miss_key, abund, flag, weight);
+    count_launches(1);
+    if ((e = exclusive_sum_u32(flag, pos, Tq, s)) != cudaSuccess) return e;
+    void* out[4] = {};
+    const size_t sizes[4] = {sizeof(u32), sizeof(u32), sizeof(u64), sizeof(u64)};
+    for (int i = 0; i < 4; ++i)
+        if ((e = cudaMallocAsync(&out[i], Tq * sizes[i], s)) != cudaSuccess) {
+            for (int j = 0; j < i; ++j) cudaFreeAsync(out[j], s);
+            return e;
+        }
+    lca_count_scatter_kernel<<<blocks, 256, 0, s>>>(key_sorted, idx_sorted, weight, flag, pos, Tq, q_off, (u32*)out[0],
+                                                    (u32*)out[1], (u64*)out[2], (u64*)out[3], d_count);
+    count_launches(1);
+    if ((e = read_count(d_count, out_n, out, 4, s)) != cudaSuccess) return e;
+    *out_q = (u32*)out[0]; *out_node = (u32*)out[1]; *out_w = (u64*)out[2]; *out_first = (u64*)out[3];
     return cudaSuccess;
 }
 

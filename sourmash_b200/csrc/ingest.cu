@@ -681,6 +681,55 @@ std::string parse_signature_json(const char* text, size_t len, uint32_t file_ind
     return J.err;
 }
 
+std::string parse_lca_hashvals(const char* text, size_t len, std::vector<uint64_t>& hashes, std::vector<uint32_t>& idx,
+                               int64_t* begin, int64_t* end) {
+    Json J{text, text + len, ""};
+    *begin = *end = -1;
+    std::string key;
+    if (!J.expect('{')) return J.err;
+    if (!J.lit('}')) for (;;) {
+        if (!J.string(key) || !J.expect(':')) return J.err;
+        if (key != "hashval_to_idx") {
+            if (!J.skip()) return J.err;
+        } else {
+            J.ws();
+            *begin = J.p - text;
+            if (!J.expect('{')) return J.err;
+            if (!J.lit('}')) for (;;) {
+                std::string hk;
+                if (!J.string(hk) || !J.expect(':')) return J.err;
+                uint64_t h = 0;
+                if (hk.empty() || hk.size() > 20) return "hash key is not a 64-bit unsigned integer";
+                for (char c : hk) {
+                    if (c < '0' || c > '9') return "hash key is not a 64-bit unsigned integer";
+                    const uint64_t d = (uint64_t)(c - '0');
+                    if (h > (UINT64_MAX - d) / 10) return "hash key is not a 64-bit unsigned integer";
+                    h = h * 10 + d;
+                }
+                if (!J.expect('[')) return J.err;
+                if (!J.lit(']')) for (;;) {
+                    uint64_t v;
+                    if (!J.u64(v)) return J.err;
+                    if (v > UINT32_MAX) return "idx out of range";
+                    hashes.push_back(h);
+                    idx.push_back((uint32_t)v);
+                    if (J.lit(',')) continue;
+                    if (!J.expect(']')) return J.err;
+                    break;
+                }
+                if (J.lit(',')) continue;
+                if (!J.expect('}')) return J.err;
+                break;
+            }
+            *end = J.p - text;
+        }
+        if (J.lit(',')) continue;
+        if (!J.expect('}')) return J.err;
+        break;
+    }
+    return J.err;
+}
+
 // md5 of one parsed sketch, the identity manifests list (KmerMinHash::md5sum, minhash.rs:290-307:
 // the decimal ksize followed by every hash in decimal)
 std::string sketch_md5(uint32_t ksize, const uint64_t* mins, size_t n) {

@@ -71,4 +71,11 @@ std::string sketch_md5(uint32_t ksize, const uint64_t* mins, size_t n);
 // Same from memory (one document).
 std::string parse_signature_json(const char* text, size_t len, uint32_t file_index, SigBatch& out);
 
+// The "hashval_to_idx" member of an LCA database's top-level JSON object ({"<hash>": [idx, ...], ...}, the only large
+// table of the format; LCA_Database.load, lca_db.py:384-391) as one (hash, idx) pair per listed idx, in file order.
+// *begin / *end: the byte span of the member's value, so that the caller can parse the rest of the document without
+// it; both -1 when the object has no such member.  Other members are scanned over, not kept.
+std::string parse_lca_hashvals(const char* text, size_t len, std::vector<uint64_t>& hashes, std::vector<uint32_t>& idx,
+                               int64_t* begin, int64_t* end);
+
 }  // namespace smb

@@ -59,6 +59,22 @@ cudaError_t sketchset_combine(const uint64_t* h, const uint64_t* abund, uint64_t
                               uint64_t max_key, uint32_t op, uint64_t** out_h, uint64_t** out_v, uint64_t* out_n,
                               cudaStream_t s);
 
+// Taxonomic LCA table and per-query LCA counts (lca_kernels.cuh).  The trie is parent[] / depth[] over n_nodes nodes,
+// node 0 the root, parent[i] < i.  lca_table_build: the n (hash, node) pairs of every database (LCA_NO_NODE: the
+// pair contributes nothing), sorted by hash, every run of equal hashes <= max_hash folded into its LCA node; *out_h
+// (sorted, distinct) and *out_lca are device arrays of *out_n entries the caller frees with cudaFreeAsync.
+// lca_counts: for the CSR of n_q queries (Tq elements), every distinct (query, LCA node) of the hashes the table
+// holds, with the summed weights (abund[e], or 1 per element without abund) and the smallest element position in the
+// query; rows ordered by (query, node), in device arrays of *out_n entries freed by the caller.  Both refuse more than
+// 2^31 - 1 elements with cudaErrorInvalidValue (cub's scan counts in int).
+constexpr uint32_t LCA_NO_NODE = 0xffffffffu;
+cudaError_t lca_table_build(const uint64_t* h, const uint32_t* nodes, uint64_t n, uint64_t max_hash, uint64_t max_key,
+                            const uint32_t* parent, const uint8_t* depth, uint64_t** out_h, uint32_t** out_lca,
+                            uint64_t* out_n, cudaStream_t s);
+cudaError_t lca_counts(const uint64_t* t_h, const uint32_t* t_lca, uint64_t n_t, const uint64_t* qh,
+                       const uint64_t* q_off, uint32_t n_q, uint64_t Tq, const uint64_t* abund, uint32_t** out_q,
+                       uint32_t** out_node, uint64_t** out_w, uint64_t** out_first, uint64_t* out_n, cudaStream_t s);
+
 // Range-major copy of a resident set and the streaming one-vs-many pass over it (range_kernels.cuh): the key
 // space is cut into P equal ranges, part p of the copy holds every row's elements of range p back to back, CTA p
 // keeps a Bloom bitmap of the query keys of its range in shared memory and streams its part.  range_major_build
