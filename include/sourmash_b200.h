@@ -518,6 +518,27 @@ const uint64_t *smb_lca_counts_count(const SmbLcaCounts *c);
 const uint64_t *smb_lca_counts_first(const SmbLcaCounts *c);
 void smb_lca_counts_free(SmbLcaCounts *c);
 
+/* Building an LCA database (`lca index`; the reference's per-pair insert and json.dump are lca/lca_db.py:145-205,
+ * 420-465).  Row r of `sigs` (the resident, downsampled sketches) is idx r.
+ * smb_lca_index_build: every hash's idx grouped on the device.  Keys in the reference's order (first insertion:
+ * rows in order, hashes ascending within a row), each key's idx ascending.  An empty set: no keys, no launch.
+ * smb_lca_index_copy: hashes[len], offsets[len + 1] (key k's idx are idx[offsets[k] .. offsets[k + 1])), idx[pairs].
+ * smb_lca_index_text: the JSON text of "hashval_to_idx" as json.dump writes it ({"<hash>": [i, ...], ...}), in key
+ * ranges: from first_key, the longest range of whole keys whose text fits max_bytes (at least one key), with the
+ * opening brace when first_key is 0 and the closing one when the range ends at len, both counted in max_bytes.  On
+ * entry *n_bytes is the capacity of out (ignored when out is null); the text is written when it fits, else nothing
+ * is.  On return *n_bytes is the range's size, so a caller whose buffer was too small (only a single key longer than
+ * max_bytes can need more) calls again with a larger one.  Returns the next key.  With no keys the one range
+ * (first_key 0) is "{}" and the next key is 0. */
+typedef struct SmbLcaIndex SmbLcaIndex;
+SmbLcaIndex *smb_lca_index_build(const SmbSketchSet *sigs);
+uintptr_t smb_lca_index_len(const SmbLcaIndex *x);                        /* distinct hashes */
+uintptr_t smb_lca_index_pairs(const SmbLcaIndex *x);                      /* (hash, idx) pairs */
+void smb_lca_index_copy(const SmbLcaIndex *x, uint64_t *hashes, uint64_t *offsets, uint32_t *idx);
+uintptr_t smb_lca_index_text(const SmbLcaIndex *x, uintptr_t first_key, uintptr_t max_bytes, char *out,
+                             uintptr_t *n_bytes);
+void smb_lca_index_free(SmbLcaIndex *x);
+
 /* Signature objects straight from a sketch set (the tail of _compute_individual,
  * command_sketch.py:770-789): signature g owns rows [g * n_ksizes, (g + 1) * n_ksizes); ksizes
  * are the ABI values.  Array freed with signatures_array_free, objects with signature_free. */
@@ -547,6 +568,11 @@ SmbSigs *smb_sigs_read(const char *const *paths, uintptr_t n_paths, int32_t n_th
  * every member, not only *.sig / *.sig.gz (traverse_yield_all=True) */
 SmbSigs *smb_sigs_read_opts(const char *const *paths, uintptr_t n_paths, int32_t n_threads,
                             uint32_t flags);
+/* the same, where a path with loose[i] != 0 is read as one JSON signature file whatever its contents and contributes
+ * nothing when it cannot be read or parsed: the files a directory holds besides *.sig / *.sig.gz, which the
+ * reference tries and skips on error when forced (MultiIndex.load_from_directory, index/__init__.py:1033-1045) */
+SmbSigs *smb_sigs_read_loose(const char *const *paths, uintptr_t n_paths, int32_t n_threads, uint32_t flags,
+                             const uint8_t *loose);
 SmbSigs *smb_sigs_parse(const char *data, uintptr_t len);          /* JSON text or gzip of it */
 /* the same batch from objects already in memory (first sketch of every signature, like
  * SourmashSignature.minhash): N sketches out of N objects in one call instead of

@@ -483,6 +483,71 @@ def lca_counts(table, query_hashes, offsets=None, weights=None):
         lib.smb_lca_counts_free(p)
 
 
+class LcaIndex:
+    """Every hash of a resident set grouped with the idx (rows) that hold it, on the GPU (``lca_index``): keys in the
+    order LCA_Database.insert first saw them, each key's idx ascending."""
+
+    def __init__(self, ptr):
+        self._ptr = ptr
+
+    def __del__(self):
+        p, self._ptr = getattr(self, "_ptr", None), None
+        if p and lib is not None:
+            lib.smb_lca_index_free(p)
+
+    def __len__(self):
+        return int(lib.smb_lca_index_len(self._ptr))
+
+    def pairs(self):
+        return int(lib.smb_lca_index_pairs(self._ptr))
+
+    def arrays(self):
+        "(hashes in key order, offsets (len + 1), idx) as numpy arrays: key k's idx are idx[offsets[k]:offsets[k + 1]]"
+        n, m = len(self), self.pairs()
+        h, off, ix = np.zeros(n, np.uint64), np.zeros(n + 1, np.uint64), np.zeros(m, np.uint32)
+        rustcall(lib.smb_lca_index_copy, self._ptr, _ptr(h, "uint64_t *"), _ptr(off, "uint64_t *"),
+                 _ptr(ix, "uint32_t *"))
+        return h, off, ix
+
+    def _ranges(self, max_bytes):
+        """memoryviews of one reused buffer, each holding one key range's text while the generator is not advanced;
+        one call per range, and a second only for a key whose text alone is longer than max_bytes"""
+        n, k, first = len(self), 0, True
+        buf = bytearray(max(int(max_bytes), 2))
+        size = ffi.new("uintptr_t *")
+        while first or k < n:
+            first = False
+            size[0] = len(buf)
+            nxt = rustcall(lib.smb_lca_index_text, self._ptr, k, int(max_bytes), ffi.from_buffer(buf), size)
+            if int(size[0]) > len(buf):
+                buf = bytearray(int(size[0]))
+                size[0] = len(buf)
+                nxt = rustcall(lib.smb_lca_index_text, self._ptr, k, int(max_bytes), ffi.from_buffer(buf), size)
+            yield memoryview(buf)[:int(size[0])]
+            k = int(nxt)
+
+    def text_chunks(self, max_bytes=256 << 20):
+        """The JSON text of "hashval_to_idx" (json.dump's form, braces included) as bytes, in ranges of whole keys of
+        at most ``max_bytes`` each, braces counted (a key longer than that is one range alone)."""
+        for view in self._ranges(max_bytes):
+            yield bytes(view)
+
+    def write_text(self, fh, max_bytes=256 << 20):
+        "the text of text_chunks written to the binary file handle ``fh`` through one buffer; returns the bytes written"
+        total = 0
+        for view in self._ranges(max_bytes):
+            fh.write(view)
+            total += len(view)
+        return total
+
+
+def lca_index(sset):
+    """Group every hash of the resident ``SketchSet`` (row r is idx r) with the rows holding it, on the device: the
+    reference's LCA_Database.insert loop over the rows in order, with hashval_to_idx's keys in its first-insertion
+    order.  Returns an ``LcaIndex``."""
+    return LcaIndex(rustcall(lib.smb_lca_index_build, sset._ptr))
+
+
 def gather(query, db, threshold=1, max_rounds=None):
     """Iterative min-set-cover; returns (match_ids, intersect_sizes) in pick order."""
     q = _u64(query)

@@ -3380,6 +3380,83 @@ const uint64_t* smb_lca_counts_count(const SmbLcaCounts* c) { return c->count.da
 const uint64_t* smb_lca_counts_first(const SmbLcaCounts* c) { return c->first.data(); }
 void smb_lca_counts_free(SmbLcaCounts* c) { delete c; }
 
+// `lca index` (lca/lca_db.py:145-205, 420-465): every hash's idx grouped on the device, and the JSON text of
+// "hashval_to_idx" written there in key ranges, each copied back once
+struct SmbLcaIndex {
+    smb::LcaIndexDev d;
+    cudaStream_t s = 0;
+    ~SmbLcaIndex() {
+        void* p[5] = {d.hash, d.koff, d.idx, d.key_of, d.at};
+        for (void* q : p) if (q) cudaFreeAsync(q, s);
+    }
+};
+
+SmbLcaIndex* smb_lca_index_build(const SmbSketchSet* sigs) {
+    return guarded<SmbLcaIndex*>([&]() -> SmbLcaIndex* {
+        const std::vector<uint64_t>& off = sigs->h_off;
+        if (sigs->n_rows > 0xffffffffull) fail(SOURMASH_ERROR_CODE_MSG, "too many signatures (idx is 32-bit)");
+        if (!off.empty() && off[0] != 0) fail(SOURMASH_ERROR_CODE_MSG, "row offsets must start at 0");
+        for (size_t i = 1; i < off.size(); ++i)
+            if (off[i] < off[i - 1]) fail(SOURMASH_ERROR_CODE_MSG, "row offsets decrease at " + std::to_string(i));
+        const uint64_t T = sigs->total();
+        if (T > 0x7ffffffeull) fail(SOURMASH_ERROR_CODE_MSG, "LCA index too large (more than 2^31 - 2 pairs)");
+        auto x = std::make_unique<SmbLcaIndex>();
+        if (T == 0) return x.release();
+        cudaStream_t s = need_gpu();
+        x->s = s;
+        const uint64_t max_key = set_max_key(*sigs, s);
+        if (t_profiling) t_timer_hash.begin(s);
+        CK(smb::lca_index_build(sigs->d_hashes, sigs->d_off, (uint32_t)sigs->n_rows, T, max_key, &x->d, s));
+        if (t_profiling) t_timer_hash.end(s);
+        return x.release();
+    });
+}
+uintptr_t smb_lca_index_len(const SmbLcaIndex* x) { return x->d.K; }
+uintptr_t smb_lca_index_pairs(const SmbLcaIndex* x) { return x->d.T; }
+void smb_lca_index_copy(const SmbLcaIndex* x, uint64_t* hashes, uint64_t* offsets, uint32_t* idx) {
+    guarded_void([&] {
+        const uint64_t K = x->d.K, T = x->d.T;
+        offsets[0] = 0;
+        if (K == 0) return;
+        std::vector<uint32_t> koff(K + 1);
+        CK(cudaMemcpyAsync(hashes, x->d.hash, K * sizeof(uint64_t), cudaMemcpyDeviceToHost, x->s));
+        CK(cudaMemcpyAsync(koff.data(), x->d.koff, (K + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, x->s));
+        CK(cudaMemcpyAsync(idx, x->d.idx, T * sizeof(uint32_t), cudaMemcpyDeviceToHost, x->s));
+        sync(x->s);
+        for (uint64_t k = 0; k <= K; ++k) offsets[k] = koff[k];
+    });
+}
+uintptr_t smb_lca_index_text(const SmbLcaIndex* x, uintptr_t first_key, uintptr_t max_bytes, char* out,
+                             uintptr_t* n_bytes) {
+    return guarded<uintptr_t>([&]() -> uintptr_t {
+        const uint64_t K = x->d.K;
+        if (K == 0) {
+            if (first_key != 0) fail(SOURMASH_ERROR_CODE_MSG, "first key out of range (the index has no keys)");
+            if (out && *n_bytes >= 2) { out[0] = '{'; out[1] = '}'; }
+            *n_bytes = 2;
+            return 0;
+        }
+        if (first_key >= K) fail(SOURMASH_ERROR_CODE_MSG, "first key " + std::to_string(first_key) + " out of range");
+        uint64_t plan[4];
+        CK(smb::lca_index_plan(x->d, first_key, max_bytes, plan, x->s));
+        const uint64_t next = plan[0], lead = first_key == 0, trail = next == K;
+        const uint64_t size = plan[1] + lead + trail;
+        if (out && *n_bytes >= size) {                                 // the range fits the caller's buffer
+            DevBuf<char> d_out(plan[1], x->s);
+            if (t_profiling) t_timer_hash.begin(x->s);
+            CK(smb::lca_index_text(x->d, plan[2], plan[3], d_out.p, x->s));
+            if (t_profiling) t_timer_hash.end(x->s);
+            d_out.download(out + lead, plan[1]);
+            sync(x->s);
+            if (lead) out[0] = '{';
+            if (trail) out[size - 1] = '}';
+        }
+        *n_bytes = size;
+        return next;
+    });
+}
+void smb_lca_index_free(SmbLcaIndex* x) { delete x; }
+
 // signatures straight from a sketch set (the tail of _compute_individual, command_sketch.py:770-789):
 // signature s gets rows [s * n_ksizes, (s + 1) * n_ksizes) of `set` as its sketches
 SourmashSignature** smb_signatures_from_sketchset(const SmbSketchSet* set, const uint32_t* ksizes,
@@ -3422,6 +3499,16 @@ SmbSigs* smb_sigs_read_opts(const char* const* paths, uintptr_t n_paths, int32_t
         auto r = std::make_unique<SmbSigs>();
         std::string err = smb::read_signature_files(paths, n_paths, n_threads > 0 ? n_threads : default_threads(),
                                                     flags, r->b);
+        if (!err.empty()) fail(SOURMASH_ERROR_CODE_SERDE_ERROR, err);
+        return r.release();
+    });
+}
+SmbSigs* smb_sigs_read_loose(const char* const* paths, uintptr_t n_paths, int32_t n_threads, uint32_t flags,
+                             const uint8_t* loose) {
+    return guarded<SmbSigs*>([&]() -> SmbSigs* {
+        auto r = std::make_unique<SmbSigs>();
+        std::string err = smb::read_signature_files(paths, n_paths, n_threads > 0 ? n_threads : default_threads(),
+                                                    flags, r->b, loose);
         if (!err.empty()) fail(SOURMASH_ERROR_CODE_SERDE_ERROR, err);
         return r.release();
     });

@@ -20,6 +20,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <algorithm>
 #include <memory>
@@ -1113,6 +1114,117 @@ cudaError_t lca_counts(const u64* t_h, const u32* t_lca, u64 n_t, const u64* qh,
     if ((e = read_count(d_count, out_n, out, 4, s)) != cudaSuccess) return e;
     *out_q = (u32*)out[0]; *out_node = (u32*)out[1]; *out_w = (u64*)out[2]; *out_first = (u64*)out[3];
     return cudaSuccess;
+}
+
+// The LCA database build (lca_kernels.cuh): iota, the sort, heads, a scan, runs, a flagged compaction into key order,
+// one readback (the number of keys), keys, a scan of the key sizes, elements, a scan of the element bytes.  Buffers are
+// allocated when first needed and the sorted hashes are freed once the keys have their hashes, so the peak is about
+// 44 bytes per pair plus 12 per key, the input set's 8 per pair included; 16 per pair and 12 per key stay resident.
+cudaError_t lca_index_build(const u64* h, const u64* row_off, u32 n_rows, u64 T, u64 max_key, LcaIndexDev* out,
+                            cudaStream_t s) {
+    *out = LcaIndexDev{};
+    if (T == 0) return cudaSuccess;
+    if (T > 0x7ffffffeull) return cudaErrorInvalidValue;
+    struct Owned {                                     // device memory freed on every path unless handed over
+        void* p = nullptr;
+        cudaStream_t s;
+        explicit Owned(cudaStream_t st) : s(st) {}
+        ~Owned() { if (p) cudaFreeAsync(p, s); }
+        cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes ? bytes : 16, s); }
+        void free_now() { if (p) cudaFreeAsync(p, s); p = nullptr; }
+    };
+    JoinScratch scratch(s);
+    cudaError_t e;
+    Owned keys(s), o_hash(s), o_koff(s), o_idx(s), o_key_of(s), o_at(s);
+    u32 *pos = nullptr, *head = nullptr, *rid = nullptr, *run_start = nullptr, *flat_head = nullptr;
+    unsigned long long* d_count = nullptr;
+    if ((e = keys.alloc(T * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = o_key_of.alloc(T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&pos, T * sizeof(u32))) != cudaSuccess) return e;
+    u64* sorted = (u64*)keys.p;
+    u32* pos_in = (u32*)o_key_of.p;                    // key_of is written last: until then it holds positions
+    const unsigned blocks = (unsigned)std::min<u64>((T + 255) / 256, (u64)SMB_SMS * 32);
+    lcx_iota_kernel<<<blocks, 256, 0, s>>>(pos_in, T); count_launches(1);
+    // (hash, flat position) sorted by hash; stable, so positions (and idx) ascend inside a run
+    if ((e = sort_hash_pairs(h, sorted, pos_in, pos, T, max_key, s)) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&head, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&rid, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&run_start, (T + 1) * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&flat_head, T * sizeof(u32))) != cudaSuccess) return e;
+    if ((e = scratch.alloc((void**)&d_count, 2 * sizeof(unsigned long long))) != cudaSuccess) return e;
+    if ((e = o_idx.alloc(T * sizeof(u32))) != cudaSuccess) return e;
+    lcx_head_kernel<<<blocks, 256, 0, s>>>(sorted, T, head); count_launches(1);
+    if ((e = exclusive_sum_u32(head, rid, T, s)) != cudaSuccess) return e;
+    u32* flat_run = pos_in;                                                    // the sort's input is free again
+    lcx_runs_kernel<<<blocks, 256, 0, s>>>(pos, head, rid, T, run_start, flat_run, flat_head, d_count);
+    count_launches(1);
+    u32* key_run = (u32*)o_idx.p;                      // idx is written by the elements pass, after key_run is read
+    {
+        size_t bytes = 0;
+        cub::DeviceSelect::Flagged(nullptr, bytes, flat_run, flat_head, key_run, d_count + 1, (int)T, s);
+        void* tmp = nullptr;
+        if ((e = cudaMallocAsync(&tmp, bytes ? bytes : 16, s)) != cudaSuccess) return e;
+        cub::DeviceSelect::Flagged(tmp, bytes, flat_run, flat_head, key_run, d_count + 1, (int)T, s);
+        cudaFreeAsync(tmp, s);
+        count_launches(1);
+    }
+    LcaIndexDev x{};
+    x.T = T;
+    void* none[1] = {};
+    if ((e = read_count(d_count, &x.K, none, 0, s)) != cudaSuccess) return e;
+    const u64 K = x.K;
+    if ((e = o_hash.alloc(K * sizeof(u64))) != cudaSuccess) return e;
+    if ((e = o_koff.alloc((K + 1) * sizeof(u32))) != cudaSuccess) return e;
+    x.hash = (u64*)o_hash.p;
+    x.koff = (u32*)o_koff.p;
+    u32* key_rank = flat_head;                                                 // the compaction's flags are free
+    const unsigned kblocks = (unsigned)std::min<u64>((K + 255) / 256, (u64)SMB_SMS * 32);
+    lcx_keys_kernel<<<kblocks, 256, 0, s>>>(key_run, K, run_start, sorted, key_rank, x.koff, x.hash);
+    count_launches(1);
+    keys.free_now();                                                           // the keys hold their hashes now
+    // element K of koff is scratch: the exclusive sum puts the total (= T) there whatever it holds
+    if ((e = exclusive_sum_u32(x.koff, x.koff, K + 1, s)) != cudaSuccess) return e;
+    if ((e = o_at.alloc((T + 1) * sizeof(u64))) != cudaSuccess) return e;
+    x.idx = (u32*)o_idx.p;
+    x.key_of = (u32*)o_key_of.p;
+    x.at = (u64*)o_at.p;
+    lcx_elems_kernel<<<blocks, 256, 0, s>>>(x.hash, pos, head, rid, T, run_start, key_rank, x.koff, row_off, n_rows,
+                                            x.idx, x.key_of, x.at);
+    count_launches(1);
+    {
+        size_t bytes = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, bytes, x.at, x.at, (int)(T + 1), s);
+        void* tmp = nullptr;
+        if ((e = cudaMallocAsync(&tmp, bytes ? bytes : 16, s)) != cudaSuccess) return e;
+        cub::DeviceScan::ExclusiveSum(tmp, bytes, x.at, x.at, (int)(T + 1), s);    // at[T]: the text's size
+        cudaFreeAsync(tmp, s);
+        count_launches(1);
+    }
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    o_hash.p = o_koff.p = o_idx.p = o_key_of.p = o_at.p = nullptr;             // handed over to the caller
+    *out = x;
+    return cudaSuccess;
+}
+
+cudaError_t lca_index_plan(const LcaIndexDev& x, u64 k0, u64 max_bytes, u64 plan[4], cudaStream_t s) {
+    unsigned long long* d = nullptr;
+    cudaError_t e = cudaMallocAsync((void**)&d, 4 * sizeof(unsigned long long), s);
+    if (e != cudaSuccess) return e;
+    lcx_plan_kernel<<<1, 1, 0, s>>>(x.at, x.koff, x.K, k0, max_bytes, d); count_launches(1);
+    unsigned long long v[4] = {0, 0, 0, 0};
+    cudaMemcpyAsync(v, d, sizeof v, cudaMemcpyDeviceToHost, s);
+    cudaFreeAsync(d, s);
+    if ((e = cudaStreamSynchronize(s)) != cudaSuccess || (e = cudaGetLastError()) != cudaSuccess) return e;
+    for (int i = 0; i < 4; ++i) plan[i] = v[i];
+    return cudaSuccess;
+}
+
+cudaError_t lca_index_text(const LcaIndexDev& x, u64 d0, u64 d1, char* out, cudaStream_t s) {
+    if (d1 <= d0) return cudaSuccess;
+    const unsigned blocks = (unsigned)std::min<u64>((d1 - d0 + 255) / 256, (u64)SMB_SMS * 32);
+    lcx_text_kernel<<<blocks, 256, 0, s>>>(x.hash, x.koff, x.idx, x.key_of, x.at, d0, d1, out);
+    count_launches(1);
+    return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------

@@ -793,7 +793,8 @@ struct SigTask { uint32_t path; const ZipMember* member; const ZipInput* zin; };
 
 }  // namespace
 
-std::string read_signature_files(const char* const* paths, size_t n_paths, int n_threads, uint32_t flags, SigBatch& out) {
+std::string read_signature_files(const char* const* paths, size_t n_paths, int n_threads, uint32_t flags, SigBatch& out,
+                                 const uint8_t* loose) {
     // 1. classify: a .zip collection expands into one task per member, in the order the reference
     //    visits them -- the manifest's distinct locations when SOURMASH-MANIFEST.csv exists
     //    (index/__init__.py:644-657), else every member named *.sig / *.sig.gz in directory
@@ -802,6 +803,7 @@ std::string read_signature_files(const char* const* paths, size_t n_paths, int n
     std::vector<SigTask> tasks;
     tasks.reserve(n_paths);
     for (size_t i = 0; i < n_paths; ++i) {
+        if (loose && loose[i]) { tasks.push_back({(uint32_t)i, nullptr, nullptr}); continue; }
         unsigned char magic[4] = {0, 0, 0, 0};
         FILE* fh = fopen(paths[i], "rb");
         if (!fh) return std::string("cannot open ") + paths[i];
@@ -853,6 +855,7 @@ std::string read_signature_files(const char* const* paths, size_t n_paths, int n
                     errs[t] = parse_signature_json((const char*)data.data(), data.size(), T.path, parts[t]);
                     if (!errs[t].empty()) errs[t] = std::string(path) + ": " + errs[t];
                 }
+                if (!errs[t].empty() && loose && loose[T.path]) { errs[t].clear(); parts[t] = SigBatch(); }
                 continue;
             }
             raw.clear(); text.clear();

@@ -64,8 +64,10 @@ enum : uint32_t {
     SIGS_NO_ZIP = 4,        // every path is one (possibly compressed) JSON file: a .zip archive is a parse error, as it is for
                             // the reference's Signature::from_path (signature.rs:569-590) behind signatures_load_path
 };
+// optional: a path i with loose[i] != 0 is read as one JSON file whatever its contents, and contributes nothing when
+// it cannot be read or parsed (MultiIndex.load_from_directory with force, index/__init__.py:1033-1045)
 std::string read_signature_files(const char* const* paths, size_t n_paths, int n_threads, uint32_t flags,
-                                 SigBatch& out);
+                                 SigBatch& out, const uint8_t* loose = nullptr);
 // md5 identity of a sketch (KmerMinHash::md5sum, minhash.rs:290-307)
 std::string sketch_md5(uint32_t ksize, const uint64_t* mins, size_t n);
 // Same from memory (one document).

@@ -75,6 +75,27 @@ cudaError_t lca_counts(const uint64_t* t_h, const uint32_t* t_lca, uint64_t n_t,
                        const uint64_t* q_off, uint32_t n_q, uint64_t Tq, const uint64_t* abund, uint32_t** out_q,
                        uint32_t** out_node, uint64_t** out_w, uint64_t** out_first, uint64_t* out_n, cudaStream_t s);
 
+// The LCA database build (`lca index`, lca_kernels.cuh) over a resident set of n_rows rows (row r is idx r) and T
+// elements.  Device arrays, freed by the caller with cudaFreeAsync: hash[K] the distinct hashes in the reference's key
+// order (first insertion), koff[K + 1] each key's first element, idx[T] the idx of the elements in key order
+// (ascending within a key), key_of[T] each element's key, at[T + 1] each element's first byte in the JSON text of
+// "hashval_to_idx" without its braces (at[T]: the text's size).  More than 2^31 - 2 elements: cudaErrorInvalidValue.
+// lca_index_plan: from key k0, the longest key range of at most max_bytes, braces included (at least one key):
+// plan = {k1, bytes without braces, first element, end element}.  lca_index_text: the text of elements [d0, d1),
+// whole keys, into device memory.
+struct LcaIndexDev {
+    uint64_t* hash = nullptr;
+    uint32_t* koff = nullptr;
+    uint32_t* idx = nullptr;
+    uint32_t* key_of = nullptr;
+    uint64_t* at = nullptr;
+    uint64_t K = 0, T = 0;
+};
+cudaError_t lca_index_build(const uint64_t* h, const uint64_t* row_off, uint32_t n_rows, uint64_t T, uint64_t max_key,
+                            LcaIndexDev* out, cudaStream_t s);
+cudaError_t lca_index_plan(const LcaIndexDev& x, uint64_t k0, uint64_t max_bytes, uint64_t plan[4], cudaStream_t s);
+cudaError_t lca_index_text(const LcaIndexDev& x, uint64_t d0, uint64_t d1, char* out, cudaStream_t s);
+
 // Range-major copy of a resident set and the streaming one-vs-many pass over it (range_kernels.cuh): the key
 // space is cut into P equal ranges, part p of the copy holds every row's elements of range p back to back, CTA p
 // keeps a Bloom bitmap of the query keys of its range in shared memory and streams its part.  range_major_build

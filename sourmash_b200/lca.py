@@ -1,5 +1,5 @@
-"""`sourmash scripts b200lcaclassify | b200lcasummarize`: taxonomic classification against LCA databases, each hash's
-lowest common ancestor found on the GPU.
+"""`sourmash scripts b200lcaclassify | b200lcasummarize | b200lcaindex`: taxonomic classification against LCA
+databases, each hash's lowest common ancestor found on the GPU, and building those databases.
 
 The reference's `sourmash lca classify` and `lca summarize` (src/sourmash/lca/command_classify.py,
 command_summarize.py) look every query hash up in every database and build a dictionary tree of its lineages to find
@@ -14,8 +14,20 @@ large "hashval_to_idx" table is parsed natively into arrays.  SQLite LCA databas
 
     sourmash scripts b200lcaclassify --db db1.lca.json db2.lca.json.gz --query q1.sig q2.sig -o out.csv
     sourmash scripts b200lcasummarize --db db.lca.json --query metagenome.sig --ignore-abundance -o out.csv
+    sourmash scripts b200lcaindex taxonomy.csv db.lca.json genomes/ -C 3 --split-identifiers --report report.txt
 
-Also ``python -m sourmash_b200.lca classify|summarize ...``.  The command classes are not yet declared as
+`lca index` (src/sourmash/lca/command_index.py) inserts every (hash, genome) pair into a dict of sets and json.dumps
+it.  Here the spreadsheet and the per-signature loop run over metadata only; the kept sketches go to the device once,
+where every hash's genomes are grouped in the reference's key order and the "hashval_to_idx" text is written in key
+ranges of bounded size (``batch.lca_index``), spliced into what Python's json writes for the other members.  Each idx
+list is ascending, where the reference writes CPython's set order (the same whenever every idx is below 8).  A
+--from-file list is read in file order; the reference reads it into a set (load_pathlist_from_file,
+sourmash_args.py:380-399), so with several entries its idx order follows the string hash seed.  Every input file is
+parsed once, before the per-signature loop, where the reference streams them file by file: a file that fails to parse
+stops the command before an error the reference would report for an earlier file (--fail-on-missing-taxonomy, a num
+sketch).  -F sql and picklists are refused.
+
+Also ``python -m sourmash_b200.lca classify|summarize|index ...``.  The command classes are not yet declared as
 ``sourmash.cli_script`` entry points in pyproject.toml, whose declared list the test suite pins to the six existing
 commands; ``sourmash scripts ...`` finds them once they are.  Report lines, CSV columns and exit codes are the
 reference's; -d/--debug is accepted but prints no debugging output.
@@ -445,7 +457,304 @@ class Command_B200LcaSummarize(CommandLinePlugin):
         return 0
 
 
-_COMMANDS = {"classify": Command_B200LcaClassify, "summarize": Command_B200LcaSummarize}
+# ---------------------------------------------------------------------------------------------------- lca index
+def filter_null(x):
+    "filter_null (lca_utils.py:128-131)"
+    return "unassigned" if x is None or x.strip() in ("[Blank]", "na", "null", "") else x
+
+
+def load_taxonomy_assignments(filename, *, delimiter=",", start_column=2, use_headers=True, force=False,
+                              split_identifiers=False, keep_identifier_versions=False):
+    """load_taxonomy_assignments (lca/command_index.py:19-127): identifier -> lineage, a tuple of (rank, name, None)
+    triples (LineagePair's fields, as json.dump writes them), and the number of non-empty rows"""
+    fp = open(filename, newline="")
+    r = csv.reader(fp, delimiter=delimiter)
+    row_headers = ["identifiers"] + ["_skip_"] * (start_column - 2) + list(TAXLIST)
+    if use_headers:
+        _notify_end("examining spreadsheet headers...", "\n")
+        first_row = next(iter(r))
+        n_disagree = 0
+        for column, value in zip(row_headers, first_row):
+            if column == "_skip_":
+                continue
+            if column.lower() != value.lower():
+                _notify_end(f"** assuming column '{value}' is {column} in spreadsheet", "\n")
+                n_disagree += 1
+                if n_disagree > 2:
+                    _error("whoa, too many assumptions. are the headers right?")
+                    _error("expecting {}".format(",".join(row_headers)))
+                    if not force:
+                        sys.exit(-1)
+                    _notify_end("...continue, because --force was specified.", "\n")
+    assignments = {}
+    num_rows = n_species = 0
+    for row in r:
+        if row and row[0].strip():
+            num_rows += 1
+            lineage = [x for x in zip(row_headers, row) if x[0] != "_skip_"]
+            ident = lineage[0][1]
+            lineage = lineage[1:]
+            if split_identifiers:
+                ident = ident.split(" ")[0]
+                if not keep_identifier_versions:
+                    ident = ident.split(".")[0]
+            lineage = [(a, filter_null(b), None) for (a, b) in lineage]
+            while lineage and lineage[-1][1] == "unassigned":
+                lineage = lineage[:-1]
+            if lineage:
+                if ident in assignments:
+                    if assignments[ident] != tuple(lineage) and not force:
+                        raise Exception(f"multiple lineages for identifier {ident}")
+                else:
+                    assignments[ident] = tuple(lineage)
+                    if lineage[-1][0] in ("species", "strain"):
+                        n_species += 1
+    fp.close()
+    if len(assignments) * 0.2 > n_species and len(assignments) > 50 and not force:
+        _error("")
+        _error("ERROR: fewer than 20% of lineages have species-level resolution!?")
+        _error("({} species assignments found, of {} assignments total)".format(n_species, len(assignments)))
+        _error("** If this is intentional, re-run the command with -f.")
+        sys.exit(-1)
+    return assignments, num_rows
+
+
+def generate_report(record_duplicates, record_no_lineage, record_remnants, unused_lineages, unused_identifiers,
+                    filename):
+    """generate_report (lca/command_index.py:130-163).  The reference lists its sets in set iteration order, which
+    varies with the string hash seed; here they are sorted."""
+    with open(filename, "w") as fp:
+        print(f"Duplicate signatures: {len(record_duplicates)}", file=fp)
+        fp.write("\n".join(sorted(record_duplicates)))
+        fp.write("\n")
+        print(f"----\nUnused identifiers: {len(unused_identifiers)}", file=fp)
+        fp.write("\n".join(sorted(unused_identifiers)))
+        fp.write("\n")
+        print(f"----\nNo lineage provided for these identifiers: {len(record_no_lineage)}", file=fp)
+        fp.write("\n".join(record_no_lineage))
+        fp.write("\n")
+        print(f"----\nNo signatures found for these identifiers: {len(record_remnants)}", file=fp)
+        fp.write("\n".join(sorted(record_remnants)))
+        fp.write("\n")
+        print(f"----\nUnused lineages: {len(unused_lineages)}", file=fp)
+        for lineage in sorted(unused_lineages):
+            fp.write(";".join(zip_lineage([p[:2] for p in lineage])))
+            fp.write("\n")
+
+
+def _index_files(paths, yield_all):
+    """the files load_file_as_signatures reads for each argument, the argument each came from, and whether it is read
+    loosely: a directory stands for its .sig / .sig.gz files, and with yield_all (-f) for every file below it, each
+    skipped when it does not parse, as MultiIndex.load_from_directory(force=True) skips it (index/__init__.py:
+    1033-1045).  The files are parsed once, by the caller."""
+    if not yield_all:
+        files, origin = _expand(paths)
+        return files, origin, None
+    files, origin, loose = [], [], []
+    for k, p in enumerate(paths):
+        if not os.path.isdir(p):
+            files.append(p)
+            origin.append(k)
+            loose.append(False)
+            continue
+        for root, _dirs, names in os.walk(p):
+            for name in sorted(names):
+                files.append(os.path.join(root, name))
+                origin.append(k)
+                loose.append(True)
+    return files, origin, loose
+
+
+def write_database(path, ksize, scaled, moltype, lid_to_lineage, index, ident_to_name, ident_to_idx, idx_to_lid,
+                   max_bytes=256 << 20):
+    """save_to_json (lca_db.py:420-465): json serialises every member but "hashval_to_idx", whose text the device
+    writes in key ranges of at most max_bytes, spliced in at its place; gzip (level 9) for a .gz name"""
+    head = OrderedDict([("version", "2.1"), ("type", "sourmash_lca"), ("license", "CC0"),
+                        ("ksize", ksize * 3 if moltype != "DNA" else ksize), ("scaled", scaled),
+                        ("moltype", moltype), ("lid_to_lineage", lid_to_lineage)])
+    tail = OrderedDict([("ident_to_name", ident_to_name), ("ident_to_idx", ident_to_idx),
+                        ("idx_to_lid", idx_to_lid)])
+    fp = gzip.open(path, "wb", compresslevel=9) if path.endswith(".gz") else open(path, "wb")
+    with fp:
+        fp.write(json.dumps(head)[:-1].encode("ascii") + b', "hashval_to_idx": ')
+        index.write_text(fp, max_bytes)
+        fp.write(b", " + json.dumps(tail)[1:].encode("ascii"))
+
+
+class Command_B200LcaIndex(CommandLinePlugin):
+    command = "b200lcaindex"
+    description = "create LCA database (lca index): every hash's genomes grouped and the table written on a GPU"
+
+    def __init__(self, p):
+        from .sigsetops import _moltype_args
+        super().__init__(p)
+        p.add_argument("csv", help="taxonomy spreadsheet")
+        p.add_argument("lca_db_out", help="output database name")
+        p.add_argument("signatures", nargs="*",
+                       help="signatures or directory of signatures to index (optional if provided via --from-file)")
+        p.add_argument("--from-file", help="a text file containing a list of files to load signatures from")
+        p.add_argument("--scaled", metavar="S", default=10000, type=float)
+        p.add_argument("-C", "--start-column", metavar="C", default=2, type=int,
+                       help="column at which taxonomic assignments start; default=2")
+        p.add_argument("--tabs", action="store_true", help="input spreadsheet is tab-delimited; default is commas")
+        p.add_argument("--no-headers", action="store_true", help="no headers present in taxonomy spreadsheet")
+        p.add_argument("--split-identifiers", action="store_true", help="split names in signatures on whitespace")
+        p.add_argument("--keep-identifier-versions", action="store_true", help="do not remove accession versions")
+        p.add_argument("-f", "--force", action="store_true")
+        p.add_argument("--report", help="output a report on anomalies, if any")
+        p.add_argument("--require-taxonomy", action="store_true", help="ignore signatures with no taxonomy entry")
+        p.add_argument("--fail-on-missing-taxonomy", action="store_true",
+                       help="fail quickly if taxonomy is not available for an identifier")
+        p.add_argument("-F", "--database-format", default="json", choices=["json", "sql"],
+                       help="format of output database; only 'json' is supported")
+        _moltype_args(p)
+
+    def main(self, args):
+        from .sigsetops import _moltype
+        from .sigset import SignatureSet
+        super().main(args)
+        if args.start_column < 2:
+            _error("error, --start-column cannot be less than 2")
+            sys.exit(-1)
+        _QUIET[0] = bool(args.quiet)
+        args.scaled = int(args.scaled)
+        if args.ksize is None:
+            args.ksize = 31
+        moltype = _moltype(args) or "DNA"
+        if args.database_format != "json":
+            _error("ERROR: SQLite LCA databases (-F sql) are not supported; write a JSON database "
+                   "(.lca.json or .lca.json.gz)")
+            sys.exit(-1)
+        db_outfile = args.lca_db_out
+        if not (db_outfile.endswith(".lca.json") or db_outfile.endswith(".lca.json.gz")):
+            db_outfile += ".lca.json"
+        if os.path.exists(db_outfile):
+            _error(f"ERROR: output file {db_outfile} already exists. Not overwriting.")
+            sys.exit(-1)
+        _notify_end(f"saving to LCA DB: {format(db_outfile)}", "\n")
+        _notify_end(f"Building LCA database with ksize={args.ksize} scaled={args.scaled} moltype={moltype}.", "\n")
+        assignments, num_rows = load_taxonomy_assignments(
+            args.csv, delimiter="\t" if args.tabs else ",", start_column=args.start_column,
+            use_headers=not args.no_headers, force=args.force, split_identifiers=args.split_identifiers,
+            keep_identifier_versions=args.keep_identifier_versions)
+        distinct_lineages = set(assignments.values())
+        _notify_end(f"{len(assignments)} distinct identities in spreadsheet out of {num_rows} rows.", "\n")
+        _notify_end(f"{len(distinct_lineages)} distinct lineages in spreadsheet out of {num_rows} rows.", "\n")
+
+        inp_files = list(args.signatures)
+        if args.from_file:
+            inp_files.extend(_pathlist(args.from_file))
+        files, origin, loose = _index_files(inp_files, args.force)
+        ss = SignatureSet.from_files(files, traverse_yield_all=args.force, loose=loose)
+        code = {"DNA": 1, "protein": 2, "dayhoff": 3, "hp": 4}[moltype]
+        want_k = args.ksize if moltype == "DNA" else 3 * args.ksize
+        rows = np.nonzero((ss.hash_function == code) & (ss.ksize == want_k))[0]
+        md5s = ss.md5sums() if len(rows) else []
+        qscaled = ss.python_scaled()
+
+        # the insert loop (command_index.py:248-329) over metadata: which rows become which idx
+        md5_seen, kept = set(), []
+        record_duplicates, record_no_lineage, record_remnants = set(), [], set(assignments)
+        record_used_lineages, record_used_idents = set(), set()
+        ident_to_name, ident_to_idx, idx_to_lid = {}, {}, {}
+        lineage_to_lid, lid_to_lineage = {}, {}
+        n_skipped = 0
+        for r in rows.tolist():
+            name, md5 = ss.name(r), md5s[r]
+            if md5 in md5_seen:
+                record_duplicates.add(name)
+                continue
+            md5_seen.add(md5)
+            ident = name if name else ss.filename(r)
+            orig_ident = ident
+            if args.split_identifiers:
+                ident = ident.split(" ")[0]
+                if not args.keep_identifier_versions:
+                    ident = ident.split(".")[0]
+            lineage = assignments.get(ident)
+            if lineage is None and args.require_taxonomy:
+                if args.fail_on_missing_taxonomy:
+                    _notify_end(f"ERROR: no taxonomy found for identifier '{ident}'", "\n")
+                    if args.split_identifiers:
+                        _notify_end(f"(Identifier extracted from name: '{orig_ident})')", "\n")
+                    sys.exit(-1)
+                n_skipped += 1
+                continue
+            shown = name or ss.filename(r) or md5[:8]                  # str(sig)
+            db_ident = ident or shown                                   # insert's ident (lca_db.py:176-177)
+            reason = None
+            if ss.max_hash[r] == 0 or int(qscaled[r]) > args.scaled:
+                reason = "cannot downsample signature; is it a scaled signature?"
+            elif db_ident in ident_to_name:
+                reason = f"signature '{db_ident}' is already in this LCA db."
+            if reason:
+                _error(f"ERROR: cannot insert signature '{shown}' (md5 {md5[:8]}, loaded from "
+                       f"'{inp_files[origin[int(ss.file[r])]]}') into database.")
+                _error(f"ERROR: {reason}")
+                sys.exit(-1)
+            ident_to_name[db_ident] = name
+            idx = len(ident_to_idx)
+            ident_to_idx[db_ident] = idx
+            if lineage:
+                lid = lineage_to_lid.setdefault(lineage, len(lineage_to_lid))
+                lid_to_lineage.setdefault(lid, lineage)
+                idx_to_lid[idx] = lid
+                record_remnants.remove(ident)
+                record_used_idents.add(ident)
+                record_used_lineages.add(lineage)
+            else:
+                record_no_lineage.append(ident)
+            kept.append(r)
+
+        if n_skipped:
+            _notify_end(f"... loaded {len(inp_files)} signatures; skipped {n_skipped} because of --require-taxonomy.",
+                        "\n")
+        else:
+            _notify_end(f"... loaded {len(inp_files)} signatures.", "\n")
+        if not inp_files:
+            _error("ERROR: no signatures found. ??")
+            sys.exit(1)
+        index = None
+        if kept:
+            sset = ss.to_sketchset(np.asarray(kept, dtype=np.uint32)).downsample(_get_max_hash_for_scaled(args.scaled))
+            index = B.lca_index(sset)
+            del sset
+        if index is None or len(index) == 0:
+            _error("ERROR: no hash values found - are there any signatures?")
+            sys.exit(1)
+        _notify_end(f"loaded {len(index)} hashes at ksize={args.ksize} scaled={args.scaled}", "\n")
+        _notify_end(f"{len(record_used_lineages)} assigned lineages out of {len(distinct_lineages)} distinct lineages "
+                    "in spreadsheet.", "\n")
+        unused_lineages = distinct_lineages - record_used_lineages
+        _notify_end(f"{len(record_used_idents)} identifiers used out of {len(set(assignments))} distinct identifiers "
+                    "in spreadsheet.", "\n")
+        unused_identifiers = set(assignments) - record_used_idents
+
+        write_database(db_outfile, args.ksize, args.scaled, moltype, lid_to_lineage, index, ident_to_name,
+                       ident_to_idx, idx_to_lid)
+
+        if record_duplicates or record_no_lineage or record_remnants or unused_lineages:
+            if record_duplicates:
+                _notify_end(f"WARNING: {len(record_duplicates)} duplicate signatures.", "\n")
+            if record_no_lineage:
+                _notify_end(f"WARNING: no lineage provided for {len(record_no_lineage)} signatures.", "\n")
+            if record_remnants:
+                _notify_end(f"WARNING: no signatures for {len(record_remnants)} spreadsheet rows.", "\n")
+            if unused_lineages:
+                _notify_end(f"WARNING: {len(unused_lineages)} unused lineages.", "\n")
+            if unused_identifiers:
+                _notify_end(f"WARNING: {len(unused_identifiers)} unused identifiers.", "\n")
+            if args.report:
+                _notify_end(f"generating a report and saving in '{args.report}'", "\n")
+                generate_report(record_duplicates, record_no_lineage, record_remnants, unused_lineages,
+                                unused_identifiers, args.report)
+            else:
+                _notify_end("(You can use --report to generate a detailed report.)", "\n")
+        return 0
+
+
+_COMMANDS = {"classify": Command_B200LcaClassify, "summarize": Command_B200LcaSummarize,
+             "index": Command_B200LcaIndex}
 
 
 def main(argv=None):

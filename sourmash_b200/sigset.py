@@ -46,15 +46,22 @@ class SignatureSet:
             lib.smb_sigs_free(p)
 
     @classmethod
-    def from_files(cls, paths, n_threads=0, *, use_manifest=True, traverse_yield_all=False):
+    def from_files(cls, paths, n_threads=0, *, use_manifest=True, traverse_yield_all=False, loose=None):
         """Parse .sig / .sig.gz files and .zip collections of them.  A zip contributes the members
         ZipFileLinearIndex.signatures() of the reference would yield (index/__init__.py:639-683);
-        the two keywords are that class's options."""
+        the two keywords are that class's options.  ``loose``: one flag per path; a flagged path is read as
+        one JSON file and contributes nothing when it does not parse (a forced directory's other files)."""
         paths = [str(p).encode("utf-8") for p in paths]
         keep = [ffi.new("char[]", p) for p in paths]
         arr = ffi.new("char *[]", keep)
         flags = (0 if use_manifest else 1) | (2 if traverse_yield_all else 0)
-        return cls(rustcall(lib.smb_sigs_read_opts, arr, len(paths), int(n_threads), flags))
+        if loose is None:
+            return cls(rustcall(lib.smb_sigs_read_opts, arr, len(paths), int(n_threads), flags))
+        mask = np.ascontiguousarray(loose, dtype=np.uint8)
+        if len(mask) != len(paths):
+            raise ValueError("one loose flag per path")
+        return cls(rustcall(lib.smb_sigs_read_loose, arr, len(paths), int(n_threads), flags,
+                            ffi.cast("uint8_t *", mask.ctypes.data) if len(mask) else ffi.NULL))
 
     @classmethod
     def from_objects(cls, objs):
